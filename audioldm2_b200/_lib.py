@@ -1,13 +1,14 @@
 """ctypes binding of the C-ABI in include/aldm_b200.h (+ the in-tree nvcc build).
 
 The shared library is built IN-TREE (audioldm2_b200/libaldm_b200.so) so it travels with the
-repo snapshot to the GPU box.  There is no fallback: if the library is missing or the device
-is not sm_100, every entry point raises.
+package.  There is no fallback: if the library is missing or the device
+is not sm_90 (H100), every entry point raises.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
+import shutil
 import subprocess
 import sys
 
@@ -16,11 +17,14 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libaldm_b200.so")
 SOURCES = ["gemm.cu", "prep.cu", "attention.cu", "elementwise.cu", "stft.cu", "program.cu", "engine_abi.cu", "microbench.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
+# nvcc from PATH, else from the CUDA toolkit (CUDA_HOME, default /usr/local/cuda)
+NVCC = shutil.which("nvcc") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
+
 MAX_TAPS = 16
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 # enums (keep in sync with the header; checked by tests/test_abi.py against the header text)
 GEMM_TC, GEMM_SIMT, GEMM_TC_V1 = 0, 1, 2
@@ -127,7 +131,7 @@ class EngineDesc(C.Structure):
 
 
 def build(verbose: bool = False, force: bool = False) -> str:
-    """Compile every CUDA source for sm_100a into audioldm2_b200/libaldm_b200.so (nvcc cross-compiles
+    """Compile every CUDA source for sm_90a into audioldm2_b200/libaldm_b200.so (nvcc cross-compiles
     without a GPU).  Rebuilds only when a source is newer than the library."""
     srcs = [os.path.join(CSRC, s) for s in SOURCES]
     deps = srcs + [os.path.join(CSRC, "common.cuh"), os.path.join(ROOT, "include", "aldm_b200.h")]
@@ -139,7 +143,7 @@ def build(verbose: bool = False, force: bool = False) -> str:
     for s in srcs:
         o = os.path.join(HERE, "build", os.path.basename(s) + ".o")
         objs.append(o)
-        cmd = ["nvcc"] + [f for f in NVCC_FLAGS if not f.startswith("--use_fast_math")] + ["-c", s, "-o", o]
+        cmd = [NVCC] + [f for f in NVCC_FLAGS if not f.startswith("--use_fast_math")] + ["-c", s, "-o", o]
         if verbose:
             print(" ".join(cmd))
         procs.append((cmd, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)))
@@ -149,7 +153,7 @@ def build(verbose: bool = False, force: bool = False) -> str:
             raise RuntimeError("nvcc failed: %s\n%s" % (" ".join(cmd), out.decode()))
         if verbose and out:
             print(out.decode())
-    cmd = ["nvcc", "-shared", "-o", LIB_PATH] + objs + ["-lcudart"]
+    cmd = [NVCC, "-shared", "-o", LIB_PATH] + objs + ["-lcudart"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
     if r.returncode != 0:
         raise RuntimeError("link failed: %s\n%s" % (" ".join(cmd), r.stdout.decode()))
@@ -206,7 +210,6 @@ def lib() -> C.CDLL:
         "aldm_last_error": (C.c_char_p, []),
         "aldm_device_check": (i32, [i32]),
         "aldm_debug_timeline": (i32, [vp, i32]),
-        "aldm_debug_umma_rate": (i32, [i32, i32, i32, vp, i32]),
         "aldm_debug_store_rate": (i32, [i32, i32, i32, i64, vp]),
     }
     for name, (res, args) in sig.items():
@@ -232,7 +235,7 @@ EXPORTED = ["aldm_gemm", "aldm_prep", "aldm_pack_b", "aldm_attention", "aldm_sof
             "aldm_engine_ddim_step", "aldm_engine_vae_decode", "aldm_engine_vocoder", "aldm_engine_vae_encode",
             "aldm_sizeof_engine_desc", "aldm_abi_version", "aldm_sizeof_op",
             "aldm_sizeof_gemm_desc", "aldm_offsetof_gemm", "aldm_last_error", "aldm_device_check", "aldm_debug_timeline",
-            "aldm_debug_umma_rate", "aldm_debug_store_rate"]
+            "aldm_debug_store_rate"]
 
 
 def check(rc: int, what: str = ""):

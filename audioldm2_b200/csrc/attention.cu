@@ -1,22 +1,11 @@
 // K5: fused softmax(scale * Q K^T + mask) V, head_dim 32, flash-style (no N x N score matrix in HBM;
 // the reference materialises it: attention.py:354-366).
 //
-// attention_tc_kernel (tcgen05): one CTA = 128 queries of one (batch, head); keys are streamed in
+// attention_tc_kernel (wgmma): one CTA = 128 queries of one (batch, head); keys are streamed in
 // tiles of 64.  Operands are single fp16 planes (the hi planes written by the projection GEMMs,
 // ALDM_OUT_QKV): Q, K row-major, V already transposed (keys contiguous), so every operand tile is
-// a plain cp.async copy into the same 128-byte-swizzled K-major layout the GEMM uses.  Both operands of the
-// two products are activations; rounding them to 11 bits costs 1.2e-4 of the 1e-3 waveform budget at 10 DDIM
-// steps (scripts/precision_study.py --only attn), a third of the tensor work and half the bytes of the split form.
-//   S = Q K^T       : 2 K-steps of 16                                                   -> TMEM (2 UMMAs)
-//   softmax          : 128 threads, one query row each (TMEM lane == row), online max/sum in the
-//                      log2 domain, P rounded to fp16 and written to shared memory as the A operand
-//                      (the row sum is accumulated from the unrounded fp32 values)
-//   O_tile = P V     : 4 K-steps, N = 32                                                -> TMEM (4 UMMAs)
-//   O += rescaled O_tile in registers (no TMEM read-modify-write)
-// Warp roles: 0-3 softmax/epilogue, 4 loader (cp.async + mbarrier), 5 TMEM alloc + MMA issue.
-// ~81 KB shared memory and 256 TMEM columns per CTA -> two CTAs per SM overlap each other's MMA
-// and softmax phases.
-//
+// a plain cp.async copy into the same 128-byte-swizzled K-major layout the GEMM uses.
+// attention_short_kernel: CUDA cores, for the <= 32-key cross-attention contexts.
 // attention_simt_kernel: CUDA-core checker on the same operands (validation only).
 // softmax_rows_kernel: row softmax for the VAE AttnBlock (model.py:216-217).
 #include <float.h>
@@ -29,7 +18,7 @@ namespace aldm {
 static constexpr int ATT_D = 32;
 
 // ------------------------------------------------------------------------------------------------
-// tcgen05 flash attention
+// wgmma flash attention
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
@@ -51,38 +40,36 @@ __device__ __forceinline__ void store_out_row(const aldm_attn_desc& d, long long
 }
 
 namespace atc {
-constexpr int QT = 128, KT = 64;
-// The row sums of P come from the tensor core: V^T carries a 33rd row of ones (N = 48 instead of 32: +8 cycles per instruction),
-// so column 32 of O_tile is sum_k P[q, k] -- of the fp16-ROUNDED probabilities, i.e. exactly the weights the numerator uses.
-// That removes 64 FADD per row and key tile from an instruction-bound loop.
-constexpr int VROWS = 48;
-// NS = number of K/V stages (a stage is released after P V(it), so the prefetch distance is NS - 1 tile periods; the
-// 2-stage kernel of round 1 left the softmax warps waiting for S 43% of the time).  Rows are 128 bytes in the
-// SWIZZLE_128B layout; Q and K use the first 64 bytes of each row (32 dims x fp16), V^T and P all 128 (64 keys).
-template <int NS>
-struct Cfg {
-  static constexpr int QA = 0;                           // [128][128B]  q in chunks 0..3
-  static constexpr int KB = QA + QT * 128;               // NS x [64][128B]   k in chunks 0..3
-  static constexpr int VT = KB + NS * KT * 128;          // NS x [48][128B]   v^T (64 keys per row); row 32 = ones, rows 33..47 = 0
-  static constexpr int PP = VT + NS * VROWS * 128;       // [128][128B]       p (64 keys per row)
-  static constexpr int BAR = PP + QT * 128;
-  static constexpr int SMEM = BAR + 128 + 1024;          // + barriers + round-up slack for the 1024-byte tile alignment
-};
-constexpr int TMEM_COLS = 256;                 // S double buffer: cols [0,64) / [64,128); O_tile: cols [128,176) (32 outputs + row sum + pad)
+constexpr int QT = 128, KT = 64, NS = 4;
+// Rows are 128 bytes in the SWIZZLE_128B layout; Q and K use the first 64 bytes of each row (32 dims x fp16), V^T all 128
+// (64 keys).  P never touches shared memory: the score accumulator is repacked in registers as the A operand of P V.
+constexpr int QA = 0;                           // [128][128B]
+constexpr int KB = QA + QT * 128;               // NS x [64][128B]
+constexpr int VT = KB + NS * KT * 128;          // NS x [32][128B]
+constexpr int BAR = VT + NS * ATT_D * 128;
+constexpr int SMEM = BAR + 128 + 1024;          // + barriers + round-up slack for the 1024-byte tile alignment
 }  // namespace atc
 
-template <int NS>
-__global__ void __launch_bounds__(192, 2) attention_tc_kernel(const __grid_constant__ aldm_attn_desc d) {
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+// One CTA = 128 queries of one (batch, head); keys are streamed in tiles of 64 by a loader warp (cp.async + mbarrier, NS
+// stages).  Warps 0-7 are two warpgroups of 64 queries each; per key tile a warpgroup computes
+//   S = Q K^T        (2 wgmma m64n64k16, operands in shared memory)
+//   online softmax   on the accumulator fragment: thread (warp w, lane 4 g + t) holds rows 16 w + g and 16 w + g + 8,
+//                    16 keys each; row maxima are combined over the 4 threads of a row with two shuffles
+//   O += P V         (4 wgmma m64n32k16, P as fp16 register operand, V^T from shared memory)
+// Both operands of the two products are activations; rounding them to 11 bits costs 1.2e-4 of the 1e-3 waveform budget
+// at 10 DDIM steps (scripts/precision_study.py --only attn).  The row sum is accumulated from the unrounded values.
+__global__ void __launch_bounds__(288, 2) attention_tc_kernel(const __grid_constant__ aldm_attn_desc d) {
   using namespace atc;
-  using L = Cfg<NS>;
-  constexpr int QA = L::QA, KB = L::KB, VT = L::VT, PP = L::PP;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* sm = smem_raw + (base - raw);
-  const uint32_t bar = base + L::BAR;
-  const uint32_t q_full = bar, kv_full0 = bar + 8, kv_empty0 = kv_full0 + 8 * NS, s_full0 = kv_empty0 + 8 * NS,
-                 p_full = s_full0 + 16, o_full = p_full + 8, tmem_slot = o_full + 8;
+  const uint32_t bar = base + BAR;
+  const uint32_t q_full = bar, kv_full0 = bar + 8, kv_empty0 = kv_full0 + 8 * NS;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * QT;
   const int bkv = d.kv_bmod > 0 ? b % d.kv_bmod : b;
@@ -91,119 +78,136 @@ __global__ void __launch_bounds__(192, 2) attention_tc_kernel(const __grid_const
   if (tid == 0) {
     // one arrival per WARP everywhere (per-thread arrivals on one mbarrier word serialise in the smem atomic unit)
     mbar_init(q_full, 32);
-    for (int i = 0; i < NS; ++i) { mbar_init(kv_full0 + 8 * i, 32); mbar_init(kv_empty0 + 8 * i, 1); }
-    mbar_init(s_full0, 1); mbar_init(s_full0 + 8, 1); mbar_init(p_full, 4); mbar_init(o_full, 1);
+    for (int i = 0; i < NS; ++i) { mbar_init(kv_full0 + 8 * i, 32); mbar_init(kv_empty0 + 8 * i, 8); }
     fence_barrier_init();
   }
-  if (warp == 5) { tmem_alloc(tmem_slot, TMEM_COLS); tmem_relinquish(); }
-  // rows 32..47 of every V^T stage (written once; the loader only ever overwrites rows 0..31): ones, then zeros
-  for (int i = tid; i < NS * 16 * 8; i += 192) {
-    const int st = i / 128, r = 32 + ((i >> 3) & 15);
-    const uint32_t v = r == 32 ? 0x3C003C00u : 0u;      // fp16 1.0 pairs
-    *reinterpret_cast<uint4*>(sm + VT + st * (VROWS * 128) + r * 128 + ((i & 7) << 4)) = make_uint4(v, v, v, v);
-  }
-  fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *reinterpret_cast<volatile uint32_t*>(sm + (tmem_slot - base));
-  const uint32_t tmem_S = tmem, tmem_O = tmem + 128;
   pdl_wait();
 
-  if (warp < 4) {
-    // =============================== softmax + output ===============================
-    const int row = tid, q = q0 + row;
+  if (warp < 8) {
+    // =============================== S, softmax, P V ===============================
+    const int wg = warp >> 2, g = lane >> 2, t = lane & 3;
+    const int rloc = wg * 64 + (warp & 3) * 16 + g;      // this thread's first query row in the tile (second: + 8)
     const float sl2 = d.scale * 1.4426950408889634f;
-    const uint32_t trow = (uint32_t)(warp * 32) << 16;
-    const uint32_t swz = (uint32_t)(row & 7);
-    float o[ATT_D];
-#pragma unroll
-    for (int i = 0; i < ATT_D; ++i) o[i] = 0.f;
-    float mrun = -INFINITY, lrun = 0.f;
     const float* mrow = d.mask ? d.mask + (long long)bkv * d.Nk : nullptr;
+    const uint64_t dQ = wgmma_desc_sw128(base + QA + wg * 64 * 128);
+    float o[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) o[i] = 0.f;
+    float mrun[2] = {-INFINITY, -INFINITY}, lrun[2] = {0.f, 0.f};
+    mbar_wait(q_full, 0);
     for (int it = 0; it < nt; ++it) {
-      const int k0 = it * KT;
-      mbar_wait(s_full0 + 8 * (it & 1), (it >> 1) & 1);
-      tc_fence_after();
-      float s[KT];
-      tmem_ld32(tmem_S + (it & 1) * KT + trow, reinterpret_cast<uint32_t*>(s));
-      tmem_ld32(tmem_S + (it & 1) * KT + trow + 32, reinterpret_cast<uint32_t*>(s + 32));
-      tmem_ld_wait();
-      float mnew, corr;
+      const int k0 = it * KT, st = it % NS;
+      mbar_wait(kv_full0 + 8 * st, (it / NS) & 1);
+      fence_proxy_async();          // cp.async-written tiles -> visible to the tensor core (async proxy)
+      float s[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) s[i] = 0.f;
+      const uint64_t dK = wgmma_desc_sw128(base + KB + st * (KT * 128));
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) wgmma_ss<KT>(s, dQ + 2 * ks, dK + 2 * ks, 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs<32>(s);
+      // s[4 j + 2 hr + e]: row rloc + 8 hr, key k0 + 8 j + 2 t + e
+      float mnew[2], corr[2];
       if (k0 + KT <= d.Nk && !mrow) {
         // interior tile, no mask: max on the raw scores (sl2 > 0), one FFMA + one MUFU per element
-        // four independent max / sum chains: a single chain of 64 dependent operations (4-cycle latency each) left the
-        // two softmax warps per scheduler waiting on themselves for ~500 cycles per key tile
-        float t4[4] = {s[0], s[1], s[2], s[3]};
 #pragma unroll
-        for (int j = 4; j < KT; j += 4) {
-          t4[0] = fmaxf(t4[0], s[j]); t4[1] = fmaxf(t4[1], s[j + 1]); t4[2] = fmaxf(t4[2], s[j + 2]); t4[3] = fmaxf(t4[3], s[j + 3]);
+        for (int hr = 0; hr < 2; ++hr) {
+          float tmax = s[2 * hr];
+#pragma unroll
+          for (int j = 0; j < 8; ++j) tmax = fmaxf(tmax, fmaxf(s[4 * j + 2 * hr], s[4 * j + 2 * hr + 1]));
+          tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 1));
+          tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 2));
+          mnew[hr] = fmaxf(mrun[hr], tmax * sl2);
+          corr[hr] = ex2_approx(mrun[hr] - mnew[hr]);      // mrun = -inf on the first tile -> 0
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) s[4 * j + 2 * hr + e] = ex2_approx(fmaf(s[4 * j + 2 * hr + e], sl2, -mnew[hr]));
         }
-        const float tmax = fmaxf(fmaxf(t4[0], t4[1]), fmaxf(t4[2], t4[3]));
-        mnew = fmaxf(mrun, tmax * sl2);
-        corr = ex2_approx(mrun - mnew);                  // mrun = -inf on the first tile -> 0
-#pragma unroll
-        for (int j = 0; j < KT; ++j) s[j] = ex2_approx(fmaf(s[j], sl2, -mnew));
       } else {
-        float tmax = -INFINITY;
 #pragma unroll
-        for (int j = 0; j < KT; ++j) {
-          const int key = k0 + j;
-          float v = s[j] * sl2;
-          if (key >= d.Nk) v = -INFINITY;                               // beyond the key range: excluded
-          else if (mrow && __ldg(mrow + key) != 1.0f) v = -FLT_MAX;     // masked_fill(-finfo.max), attention.py:356-360
-          s[j] = v;
-          tmax = fmaxf(tmax, v);
-        }
-        mnew = fmaxf(mrun, tmax);
-        corr = (mrun == -INFINITY) ? 0.f : ex2_approx(mrun - mnew);
+        for (int hr = 0; hr < 2; ++hr) {
+          float tmax = -INFINITY;
 #pragma unroll
-        for (int j = 0; j < KT; ++j) {
-          s[j] = (s[j] == -INFINITY) ? 0.f : ex2_approx(s[j] - mnew);
+          for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int key = k0 + 8 * j + 2 * t + e;
+              float v = s[4 * j + 2 * hr + e] * sl2;
+              if (key >= d.Nk) v = -INFINITY;                               // beyond the key range: excluded
+              else if (mrow && __ldg(mrow + key) != 1.0f) v = -FLT_MAX;     // masked_fill(-finfo.max), attention.py:356-360
+              s[4 * j + 2 * hr + e] = v;
+              tmax = fmaxf(tmax, v);
+            }
+          tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 1));
+          tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 2));
+          mnew[hr] = fmaxf(mrun[hr], tmax);
+          corr[hr] = (mrun[hr] == -INFINITY) ? 0.f : ex2_approx(mrun[hr] - mnew[hr]);
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float v = s[4 * j + 2 * hr + e];
+              s[4 * j + 2 * hr + e] = (v == -INFINITY) ? 0.f : ex2_approx(v - mnew[hr]);
+            }
         }
       }
-      mrun = mnew;
-      // Deferred accumulation: fold in O_tile of the PREVIOUS key tile (its P V product has long finished
-      // while this tile's probabilities were computed), then rescale to the new running maximum.  Waiting
-      // for o_full(it-1) here also guarantees the tensor core is done reading the P buffer we overwrite next.
-      if (it > 0) {
-        mbar_wait(o_full, (it - 1) & 1);
-        tc_fence_after();
-        float ot[ATT_D];
-        tmem_ld32(tmem_O + trow, reinterpret_cast<uint32_t*>(ot));
-        const uint32_t lt = tmem_ld1(tmem_O + trow + ATT_D);      // column 32: row sum of P(it-1)
-        tmem_ld_wait();
+      // row sums (this thread's 16 keys per row; the 4 threads of a row are combined once at the end) and O rescale
 #pragma unroll
-        for (int i = 0; i < ATT_D; ++i) o[i] = (o[i] + ot[i]) * corr;
-        lrun = (lrun + __uint_as_float(lt)) * corr;
+      for (int hr = 0; hr < 2; ++hr) {
+        float ps = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) ps += s[4 * j + 2 * hr] + s[4 * j + 2 * hr + 1];
+        lrun[hr] = lrun[hr] * corr[hr] + ps;
+        mrun[hr] = mnew[hr];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { o[4 * j + 2 * hr] *= corr[hr]; o[4 * j + 2 * hr + 1] *= corr[hr]; }
       }
-      uint8_t* ph = sm + PP + row * 128;
+      // P as the A operand (fp16): k16 chunk kc covers keys 16 kc .. 16 kc + 15 = accumulator column blocks 2 kc, 2 kc + 1
+      uint32_t pa[4][4];
 #pragma unroll
-      for (int c = 0; c < KT / 8; ++c) *reinterpret_cast<uint4*>(ph + (((uint32_t)c ^ swz) << 4)) = pack8_hi_unit(s + c * 8);
-      fence_proxy_async();          // P (generic-proxy stores) -> visible to the tensor core (async proxy)
-      tc_fence_before();
+      for (int kc = 0; kc < 4; ++kc) {
+        pa[kc][0] = pack_half2(s[8 * kc + 0], s[8 * kc + 1]);
+        pa[kc][1] = pack_half2(s[8 * kc + 2], s[8 * kc + 3]);
+        pa[kc][2] = pack_half2(s[8 * kc + 4], s[8 * kc + 5]);
+        pa[kc][3] = pack_half2(s[8 * kc + 6], s[8 * kc + 7]);
+      }
+      const uint64_t dV = wgmma_desc_sw128(base + VT + st * (ATT_D * 128));
+      wgmma_fence();
+#pragma unroll
+      for (int kc = 0; kc < 4; ++kc) wgmma_rs<ATT_D>(o, pa[kc], dV + 2 * kc, 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs<16>(o);
       __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
+      if (lane == 0) mbar_arrive(kv_empty0 + 8 * st);      // this warp's reads of stage st are complete
     }
-    {
-      mbar_wait(o_full, (nt - 1) & 1);
-      tc_fence_after();
-      float ot[ATT_D];
-      tmem_ld32(tmem_O + trow, reinterpret_cast<uint32_t*>(ot));
-      const uint32_t lt = tmem_ld1(tmem_O + trow + ATT_D);
-      tmem_ld_wait();
+    if (tid == 0) pdl_launch();
 #pragma unroll
-      for (int i = 0; i < ATT_D; ++i) o[i] += ot[i];
-      lrun += __uint_as_float(lt);
-    }
-    tc_fence_before();
-    if (q < d.Nq) {
-      const float inv = 1.0f / lrun;
+    for (int hr = 0; hr < 2; ++hr) {
+      float l = lrun[hr];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      const int q = q0 + rloc + 8 * hr;
+      if (q < d.Nq) {
+        const float inv = 1.0f / l;
+        const long long orow = (long long)b * d.Nq + q;
+        aldm_plane_t* hp = reinterpret_cast<aldm_plane_t*>(d.out_hi) + orow * d.ldo + h * ATT_D + 2 * t;
+        aldm_plane_t* lp = d.out_lo ? reinterpret_cast<aldm_plane_t*>(d.out_lo) + orow * d.ldo + h * ATT_D + 2 * t : nullptr;
 #pragma unroll
-      for (int i = 0; i < ATT_D; ++i) o[i] *= inv;
-      store_out_row(d, (long long)b * d.Nq + q, h, o);
+        for (int j = 0; j < 4; ++j) {
+          uint32_t hh, ll;
+          split2(o[4 * j + 2 * hr] * inv, o[4 * j + 2 * hr + 1] * inv, hh, ll);
+          *reinterpret_cast<uint32_t*>(hp + 8 * j) = hh;
+          if (lp) *reinterpret_cast<uint32_t*>(lp + 8 * j) = ll;
+        }
+      }
     }
-  } else if (warp == 4) {
+  } else {
     // =============================== loader ===============================
     const aldm_plane_t* qh = reinterpret_cast<const aldm_plane_t*>(d.q_hi);
     const aldm_plane_t* kh = reinterpret_cast<const aldm_plane_t*>(d.k_hi);
@@ -218,252 +222,7 @@ __global__ void __launch_bounds__(192, 2) attention_tc_kernel(const __grid_const
     cp_async_mbar_arrive_noinc(q_full);
     // K/V tiles: all row bases are hoisted out of the tile loop (the loader is a single warp: per-element 64-bit index
     // arithmetic was the bottleneck).  K: lane -> chunk ck (of 4), rows rk + 8i; V^T: lane -> chunk cv (of 8), rows rv + 4i.
-    const int ck = lane & 3, rk = lane >> 2;
-    const int cv = lane & 7, rv = lane >> 3;
-    const aldm_plane_t* kcol = kh + (long long)bkv * d.Nk * d.ldk + d.k_col + h * ATT_D + ck * 8;
-    const long long vrow0 = ((long long)(bkv * d.heads + h) * ATT_D + rv) * d.ld_t + cv * 8;
-    const long long kstep = 8ll * d.ldk, vstep = 4ll * d.ld_t;
-    for (int it = 0, s = 0, ph = 1; it < nt; ++it) {
-      const int k0 = it * KT;
-      mbar_wait(kv_empty0 + 8 * s, ph);
-      const uint32_t kb = base + KB + s * (KT * 128);
-      const aldm_plane_t* kp = kcol + (long long)(k0 + rk) * d.ldk;
-#pragma unroll
-      for (int i = 0; i < KT / 8; ++i) {
-        const int r = rk + 8 * i;
-        const bool ok = k0 + r < d.Nk;
-        cp_async_16(kb + r * 128 + ((uint32_t)(ck ^ (r & 7)) << 4), ok ? kp + i * kstep : kcol, ok ? 16u : 0u);
-      }
-      const uint32_t vb = base + VT + s * (VROWS * 128);
-      const bool vok = k0 + cv * 8 < d.Nk;
-#pragma unroll
-      for (int i = 0; i < ATT_D / 4; ++i) {
-        const int r = rv + 4 * i;
-        const aldm_plane_t* vp = vh + vrow0 + i * vstep + k0;
-        cp_async_16(vb + r * 128 + ((uint32_t)(cv ^ (r & 7)) << 4), vok ? vp : vh, vok ? 16u : 0u);
-      }
-      cp_async_mbar_arrive_noinc(kv_full0 + 8 * s);
-      if (++s == NS) { s = 0; ph ^= 1; }
-    }
-  } else {
-    // =============================== MMA issuer ===============================
-    if (elect_one()) {
-      constexpr uint32_t idS = umma_idesc_f16(128, KT), idO = umma_idesc_f16(128, VROWS);
-      const uint64_t dQ = umma_desc_sw128(base + QA);
-      const uint64_t dP = umma_desc_sw128(base + PP);
-      auto issue_S = [&](int t) {      // S(t) = Q K(t)^T into TMEM buffer t & 1
-        const int st = t % NS;
-        mbar_wait(kv_full0 + 8 * st, (t / NS) & 1);      // returns at once when the caller has already seen it complete
-        tc_fence_after();
-        const uint64_t dK = umma_desc_sw128(base + KB + st * (KT * 128));
-        const uint32_t tS = tmem_S + (t & 1) * KT;
-        // descriptor address units are 16 bytes: +2 = next K-step of 16 fp16
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) umma_f16(tS, dQ + 2 * ks, dK + 2 * ks, idS, ks > 0);
-        umma_commit(s_full0 + 8 * (t & 1));
-      };
-      mbar_wait(q_full, 0);
-      issue_S(0);
-      for (int it = 0; it < nt; ++it) {
-        const int s = it % NS;
-        // S(it+1) runs on the tensor core while the softmax warps work on S(it) (its TMEM buffer was drained
-        // before p_full(it-1), which this thread has already observed) -- but only if K(it+1) has landed:
-        // otherwise P V(it) goes first so that its stage is released and the loader keeps prefetching.
-        bool s_next = it + 1 >= nt;
-        if (!s_next && mbar_test_wait(kv_full0 + 8 * ((it + 1) % NS), ((it + 1) / NS) & 1)) { issue_S(it + 1); s_next = true; }
-        mbar_wait(p_full, it & 1);
-        tc_fence_after();
-        const uint64_t dV = umma_desc_sw128(base + VT + s * (VROWS * 128));
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) umma_f16(tmem_O, dP + 2 * ks, dV + 2 * ks, idO, ks > 0);
-        umma_commit(o_full);
-        umma_commit(kv_empty0 + 8 * s);
-        if (!s_next) issue_S(it + 1);
-      }
-      pdl_launch();     // last P V issued: schedule the next kernel's blocks under this CTA's tail
-    }
-    __syncwarp();
-  }
-  __syncthreads();
-  if (warp == 5) { tc_fence_after(); tmem_dealloc(tmem, TMEM_COLS); }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Three CTAs per SM (used for Nk <= 512).  The kernel above is a chain of latencies per key tile -- S ready -> TMEM read -> max -> exp ->
-// P stored -> P V -> O read -- with two CTAs per SM to hide them: issue slots 49 % busy, tensor pipe 10 % (profiles/r02_ncu_full.md).
-// A third resident CTA needs <= 113 registers per thread, <= 75 KB of shared memory and <= 170 TMEM columns:
-//   * the scores stay in TENSOR MEMORY and are read twice in 32-column pieces (pass 1: row maximum, pass 2: exp2 + pack), so a
-//     softmax thread holds 32 scores + 32 output accumulators instead of 64 + 32 (+ 32 transient);
-//   * S is single-buffered (columns [0,64); O_tile [64,96); 128 columns allocated): S(it+1) is issued right after the softmax warps
-//     released S(it), ahead of P V(it), so the next tile's scores are ready one short MMA (2 instructions) after the hand-over;
-//   * three K/V stages (68 KB + barriers).
-// Same arithmetic as attention_tc_kernel (the row sum is accumulated per 32-column piece).
-// ------------------------------------------------------------------------------------------------
-namespace atc3 {
-constexpr int QT = 128, KT = 64, NS = 3;
-constexpr int QA = 0;                           // [128][128B]
-constexpr int KB = QA + QT * 128;               // NS x [64][128B]
-constexpr int VT = KB + NS * KT * 128;          // NS x [32][128B]
-constexpr int PP = VT + NS * ATT_D * 128;       // [128][128B]
-constexpr int BAR = PP + QT * 128;
-constexpr int SMEM = BAR + 128 + 1024;
-constexpr int TMEM_COLS = 128;                  // S: cols [0,64); O_tile: cols [64,96)
-}  // namespace atc3
-
-__global__ void __launch_bounds__(192, 3) attention_tc3_kernel(const __grid_constant__ aldm_attn_desc d) {
-  using namespace atc3;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* sm = smem_raw + (base - raw);
-  const uint32_t bar = base + BAR;
-  const uint32_t q_full = bar, kv_full0 = bar + 8, kv_empty0 = kv_full0 + 8 * NS, s_full = kv_empty0 + 8 * NS,
-                 p_full = s_full + 8, o_full = p_full + 8, tmem_slot = o_full + 8;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * QT;
-  const int bkv = d.kv_bmod > 0 ? b % d.kv_bmod : b;
-  const int nt = (d.Nk + KT - 1) / KT;
-
-  if (tid == 0) {
-    mbar_init(q_full, 32);
-    for (int i = 0; i < NS; ++i) { mbar_init(kv_full0 + 8 * i, 32); mbar_init(kv_empty0 + 8 * i, 1); }
-    mbar_init(s_full, 1); mbar_init(p_full, 4); mbar_init(o_full, 1);
-    fence_barrier_init();
-  }
-  if (warp == 5) { tmem_alloc(tmem_slot, TMEM_COLS); tmem_relinquish(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *reinterpret_cast<volatile uint32_t*>(sm + (tmem_slot - base));
-  const uint32_t tmem_S = tmem, tmem_O = tmem + 64;
-  pdl_wait();
-
-  if (warp < 4) {
-    // =============================== softmax + output ===============================
-    const int row = tid, q = q0 + row;
-    const float sl2 = d.scale * 1.4426950408889634f;
-    const uint32_t trow = (uint32_t)(warp * 32) << 16;
-    const uint32_t swz = (uint32_t)(row & 7);
-    float o[ATT_D];
-#pragma unroll
-    for (int i = 0; i < ATT_D; ++i) o[i] = 0.f;
-    float mrun = -INFINITY, lrun = 0.f;
-    const float* mrow = d.mask ? d.mask + (long long)bkv * d.Nk : nullptr;
-    for (int it = 0; it < nt; ++it) {
-      const int k0 = it * KT;
-      const bool interior = k0 + KT <= d.Nk && !mrow;
-      mbar_wait(s_full, it & 1);
-      tc_fence_after();
-      // ---- pass 1: row maximum (scores stay in tensor memory) ----
-      float mnew;
-      {
-        float tmax = -INFINITY;
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-          float s[32];
-          tmem_ld32(tmem_S + trow + hf * 32, reinterpret_cast<uint32_t*>(s));
-          tmem_ld_wait();
-          if (interior) {
-            float t4[4] = {s[0], s[1], s[2], s[3]};
-#pragma unroll
-            for (int j = 4; j < 32; j += 4) {
-              t4[0] = fmaxf(t4[0], s[j]); t4[1] = fmaxf(t4[1], s[j + 1]); t4[2] = fmaxf(t4[2], s[j + 2]); t4[3] = fmaxf(t4[3], s[j + 3]);
-            }
-            tmax = fmaxf(tmax, fmaxf(fmaxf(t4[0], t4[1]), fmaxf(t4[2], t4[3])));
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int key = k0 + hf * 32 + j;
-              float v = s[j] * sl2;
-              if (key >= d.Nk) v = -INFINITY;                               // beyond the key range: excluded
-              else if (mrow && __ldg(mrow + key) != 1.0f) v = -FLT_MAX;     // masked_fill(-finfo.max), attention.py:356-360
-              tmax = fmaxf(tmax, v);
-            }
-          }
-        }
-        mnew = fmaxf(mrun, interior ? tmax * sl2 : tmax);      // sl2 > 0
-      }
-      const float corr = (mrun == -INFINITY) ? 0.f : ex2_approx(mrun - mnew);
-      // ---- fold in O_tile of the previous key tile, rescaled to the new maximum (also: P V(it-1) has finished reading P) ----
-      if (it > 0) {
-        mbar_wait(o_full, (it - 1) & 1);
-        tc_fence_after();
-        float ot[ATT_D];
-        tmem_ld32(tmem_O + trow, reinterpret_cast<uint32_t*>(ot));
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < ATT_D; ++i) o[i] = (o[i] + ot[i]) * corr;
-      }
-      // ---- pass 2: probabilities -> fp16 P in shared memory, row sum from the unrounded values ----
-      float psum = 0.f;
-      uint8_t* ph = sm + PP + row * 128;
-#pragma unroll
-      for (int hf = 0; hf < 2; ++hf) {
-        float s[32];
-        tmem_ld32(tmem_S + trow + hf * 32, reinterpret_cast<uint32_t*>(s));
-        tmem_ld_wait();
-        float p4[4] = {0.f, 0.f, 0.f, 0.f};
-        if (interior) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float p = ex2_approx(fmaf(s[j + e], sl2, -mnew));
-              s[j + e] = p;
-              p4[e] += p;
-            }
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int key = k0 + hf * 32 + j;
-            float v = s[j] * sl2;
-            if (key >= d.Nk) v = -INFINITY;
-            else if (mrow && __ldg(mrow + key) != 1.0f) v = -FLT_MAX;
-            const float p = (v == -INFINITY) ? 0.f : ex2_approx(v - mnew);
-            s[j] = p;
-            p4[j & 3] += p;
-          }
-        }
-        psum += (p4[0] + p4[1]) + (p4[2] + p4[3]);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) *reinterpret_cast<uint4*>(ph + (((uint32_t)(hf * 4 + c) ^ swz) << 4)) = pack8_hi_unit(s + c * 8);
-      }
-      lrun = lrun * corr + psum;
-      mrun = mnew;
-      fence_proxy_async();          // P (generic-proxy stores) -> visible to the tensor core (async proxy)
-      tc_fence_before();            // our TMEM reads of S are complete before the MMA warp overwrites it
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-    }
-    {
-      mbar_wait(o_full, (nt - 1) & 1);
-      tc_fence_after();
-      float ot[ATT_D];
-      tmem_ld32(tmem_O + trow, reinterpret_cast<uint32_t*>(ot));
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < ATT_D; ++i) o[i] += ot[i];
-    }
-    tc_fence_before();
-    if (q < d.Nq) {
-      const float inv = 1.0f / lrun;
-#pragma unroll
-      for (int i = 0; i < ATT_D; ++i) o[i] *= inv;
-      store_out_row(d, (long long)b * d.Nq + q, h, o);
-    }
-  } else if (warp == 4) {
-    // =============================== loader ===============================
-    const aldm_plane_t* qh = reinterpret_cast<const aldm_plane_t*>(d.q_hi);
-    const aldm_plane_t* kh = reinterpret_cast<const aldm_plane_t*>(d.k_hi);
-    const aldm_plane_t* vh = reinterpret_cast<const aldm_plane_t*>(d.vt_hi);
-    for (int idx = lane; idx < QT * 4; idx += 32) {
-      const int r = idx >> 2, c = idx & 3;
-      const bool ok = q0 + r < d.Nq;
-      const long long off = ok ? ((long long)b * d.Nq + q0 + r) * d.ldq + d.q_col + h * ATT_D + c * 8 : 0;
-      cp_async_16(base + QA + r * 128 + ((uint32_t)(c ^ (r & 7)) << 4), qh + off, ok ? 16u : 0u);
-    }
-    cp_async_mbar_arrive_noinc(q_full);
+    // Keys beyond Nk are zero-filled (K: finite scores that the softmax excludes; V^T: zero rows of P V).
     const int ck = lane & 3, rk = lane >> 2;
     const int cv = lane & 7, rv = lane >> 3;
     const aldm_plane_t* kcol = kh + (long long)bkv * d.Nk * d.ldk + d.k_col + h * ATT_D + ck * 8;
@@ -491,47 +250,13 @@ __global__ void __launch_bounds__(192, 3) attention_tc3_kernel(const __grid_cons
       cp_async_mbar_arrive_noinc(kv_full0 + 8 * s);
       if (++s == NS) { s = 0; ph ^= 1; }
     }
-  } else {
-    // =============================== MMA issuer ===============================
-    if (elect_one()) {
-      constexpr uint32_t idS = umma_idesc_f16(128, KT), idO = umma_idesc_f16(128, ATT_D);
-      const uint64_t dQ = umma_desc_sw128(base + QA);
-      const uint64_t dP = umma_desc_sw128(base + PP);
-      auto issue_S = [&](int t) {      // S(t) = Q K(t)^T
-        const int st = t % NS;
-        mbar_wait(kv_full0 + 8 * st, (t / NS) & 1);
-        tc_fence_after();
-        const uint64_t dK = umma_desc_sw128(base + KB + st * (KT * 128));
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) umma_f16(tmem_S, dQ + 2 * ks, dK + 2 * ks, idS, ks > 0);
-        umma_commit(s_full);
-      };
-      mbar_wait(q_full, 0);
-      issue_S(0);
-      for (int it = 0; it < nt; ++it) {
-        const int s = it % NS;
-        mbar_wait(p_full, it & 1);         // the softmax warps have read S(it) and written P(it)
-        tc_fence_after();
-        if (it + 1 < nt) issue_S(it + 1);  // scores of the next tile first: the softmax warps wait for nothing else
-        const uint64_t dV = umma_desc_sw128(base + VT + s * (ATT_D * 128));
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) umma_f16(tmem_O, dP + 2 * ks, dV + 2 * ks, idO, ks > 0);
-        umma_commit(o_full);
-        umma_commit(kv_empty0 + 8 * s);
-      }
-      pdl_launch();
-    }
-    __syncwarp();
   }
-  __syncthreads();
-  if (warp == 5) { tc_fence_after(); tmem_dealloc(tmem, TMEM_COLS); }
 }
 
 // ------------------------------------------------------------------------------------------------
 // Short key sets (cross-attention to the 8-token CLAP/GPT-2 and 32-token T5 contexts): Nk <= 32.
-// The tensor-core kernel pays its whole fixed cost (TMEM allocation, three mbarrier hand-overs, a 64-key
-// tile that is mostly padding) for ~0.1 GFLOP: 37 us per launch in the step's launch list, 32 launches
-// per DDIM step.  Here one thread owns one query, K and V of the (batch, head) sit in shared memory as
+// The tensor-core kernel would pay its whole fixed cost (mbarrier hand-overs, two MMA round trips, a 64-key
+// tile that is mostly padding) for ~0.1 GFLOP, 32 times per DDIM step.  Here one thread owns one query, K and V of the (batch, head) sit in shared memory as
 // fp32 (converted from their fp16 planes), and the 2 x Nk x 32 FMAs per query run on the CUDA cores.
 // ------------------------------------------------------------------------------------------------
 template <int NKT>
@@ -675,25 +400,14 @@ int attention_launch(const aldm_attn_desc& d, cudaStream_t st) {
     if (d.Nk <= 8) ALDM_CHECK_CUDA(launch_pdl(attention_short_kernel<8>, grid, dim3(128), 0, st, d));
     else if (d.Nk <= 16) ALDM_CHECK_CUDA(launch_pdl(attention_short_kernel<16>, grid, dim3(128), 0, st, d));
     else ALDM_CHECK_CUDA(launch_pdl(attention_short_kernel<32>, grid, dim3(128), 0, st, d));
-  } else if (d.Nk <= 512 && !(getenv("ALDM_ATTN3") && getenv("ALDM_ATTN3")[0] == '0')) {
-    // three CTAs per SM for up to 8 key tiles (measured: 13.1 vs 15.0 us at N = 256, 6.7 vs 7.9 at N = 64; at N = 1024 the second
-    // TMEM pass and the single S buffer cost more than the third CTA hides: 84.6 vs 80.8 us).  ALDM_ATTN3=0: A/B switch.
-    static bool configured3 = false;
-    if (!configured3) {
-      ALDM_CHECK_CUDA(cudaFuncSetAttribute(attention_tc3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, atc3::SMEM));
-      configured3 = true;
-    }
-    dim3 grid(cdiv(d.Nq, atc3::QT), d.heads, d.B);
-    ALDM_CHECK_CUDA(launch_pdl(attention_tc3_kernel, grid, dim3(192), atc3::SMEM, st, d));
   } else {
     static bool configured = false;
-    constexpr int NS = 4;       // 81 KB: two CTAs per SM (TMEM: 2 x 256 columns)
-    if (!configured) {
-      ALDM_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, atc::Cfg<NS>::SMEM));
+    if (!configured) {      // ~65 KB: three CTAs per SM
+      ALDM_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, atc::SMEM));
       configured = true;
     }
     dim3 grid(cdiv(d.Nq, atc::QT), d.heads, d.B);
-    ALDM_CHECK_CUDA(launch_pdl(attention_tc_kernel<NS>, grid, dim3(192), atc::Cfg<NS>::SMEM, st, d));
+    ALDM_CHECK_CUDA(launch_pdl(attention_tc_kernel, grid, dim3(288), atc::SMEM, st, d));
   }
   ALDM_CHECK_CUDA(cudaGetLastError());
   return ALDM_OK;

@@ -1,5 +1,5 @@
-// Shared device helpers for the sm_100a kernels: PTX wrappers (mbarrier, cp.async, bulk copy,
-// tcgen05 / TMEM), bf16 hi/lo splitting, error plumbing.
+// Shared device helpers for the sm_90a kernels: PTX wrappers (mbarrier, cp.async, bulk copy,
+// wgmma), fp16 hi/lo splitting, error plumbing.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -35,16 +35,15 @@ inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
 // ---- programmatic dependent launch (PDL) ----------------------------------------------------
 // Every kernel of the per-step programs is launched with programmatic stream serialisation: it may
-// start (block scheduling, barrier init, TMEM allocation, index set-up) while its predecessor drains,
-// and calls pdl_wait() before its first global-memory access, which blocks until the predecessor has
-// completed and flushed.  Because every such kernel waits, completion stays transitive along the
-// stream (kernel k+2 cannot pass its wait before kernel k is done).  pdl_launch() is issued LATE (last MMA
-// issued / last loads done): triggering at kernel entry made small dependent blocks co-resident with the
-// primary for its whole run time and measurably slowed it (+1.5 ms per DDIM step; split-K GEMM + reduction
-// pair +12 us), so the early start is limited to the primary's tail.  It must also come AFTER any TMEM
-// allocation (a dependent CTA that grabbed TMEM first could starve a still-unallocated primary CTA).
+// start (block scheduling, barrier init, index set-up) while its predecessor drains, and calls pdl_wait()
+// before its first global-memory access, which blocks until the predecessor has completed and flushed.
+// Because every such kernel waits, completion stays transitive along the stream (kernel k+2 cannot pass
+// its wait before kernel k is done).  pdl_launch() is issued LATE (last MMA issued / last loads done), so
+// that dependent blocks are co-resident with the primary only for its tail rather than its whole run.
 // ALDM_PDL=0 in the environment disables the launch attribute (the device instructions are then no-ops).
 bool pdl_enabled();
+// streaming multiprocessors of the current device (grid sizing of the persistent and grid-stride kernels)
+int num_sms();
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
@@ -121,7 +120,7 @@ __device__ __forceinline__ uint4 pack8_hi(const float* v) {
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 // erf GELU as F.gelu default (attention.py:44).  erf via Abramowitz-Stegun 7.1.26 (|err| < 5e-7 in fp32,
 // i.e. at fp32 round-off of the GELU output): 1 RCP + 1 EX2 + 8 FMA-class instructions instead of the
-// ~40-instruction erff -- the GEGLU epilogue is issue-bound (profiles/r01_gemm_timeline_tc3.txt).
+// ~40-instruction erff -- the GEGLU epilogue is issue-bound.
 __device__ __forceinline__ float gelu_f(float x) {
   const float z = fabsf(x) * 0.70710678118654752440f;
   float t;      // rcp.approx (1 MUFU, ~1 ulp): __frcp_rn expands to MUFU + Newton step + a guarded slow-path CALL per element
@@ -139,8 +138,8 @@ __device__ __forceinline__ float gelu_f(float x) {
 
 // v[i] *= gelu(g[i]) for NB values at once, written stage by stage so that NB independent dependency chains are in
 // flight: the GEGLU epilogue runs two warps per scheduler, and with the elements evaluated one or two at a time
-// (what the compiler produced from the scalar form under the 128-register cap) the ~75-cycle chain of each element
-// (two MUFU round trips) was fully exposed: 3,900 cycles per 32 x 32 chunk in the timeline, 7,000 per tile.
+// (what the compiler produces from the scalar form under the 128-register cap) the dependency chain of each element
+// (two MUFU round trips) is fully exposed.
 template <int NB>
 __device__ __forceinline__ void geglu_mul(float* __restrict__ v, const float* __restrict__ g) {
   float z[NB], t[NB], e[NB], p[NB];
@@ -202,9 +201,10 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-// Bounded wait: a protocol bug must become a CUDA error, never a hung GPU box.  The timer is only
-// consulted every 4096 failed probes (try_wait itself suspends the thread in hardware), so the
-// hot path is a bare try_wait loop.
+// Bounded wait: a protocol bug must become a CUDA error (a trap after 4 s), never a hung GPU.  The timer is
+// only consulted every 4096 failed probes (try_wait itself suspends the thread in hardware), so the hot path
+// is a bare try_wait loop.  No printf here: a call inside the wgmma consumer loops makes ptxas serialise the
+// asynchronous MMAs across it.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   uint64_t t0 = 0;
@@ -213,11 +213,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if ((++spins & 4095u) == 0) {
       const uint64_t now = globaltimer_ns();
       if (t0 == 0) t0 = now;
-      else if (now - t0 > 4000000000ull) {   // 4 s
-        printf("aldm: mbarrier wait timeout (block %d,%d,%d thread %d bar %u parity %u)\n", blockIdx.x, blockIdx.y,
-               blockIdx.z, threadIdx.x, bar, parity);
-        __trap();
-      }
+      else if (now - t0 > 4000000000ull) __trap();   // 4 s
     }
   }
 }
@@ -238,7 +234,7 @@ __device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_wait_spin(uint32_t bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_test_wait(bar, parity)) {
-    if (++spins > (1u << 28)) { printf("aldm: mbarrier spin timeout\n"); __trap(); }
+    if (++spins > (1u << 28)) __trap();
   }
 }
 
@@ -276,11 +272,8 @@ __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// One elected lane of a fully converged warp.  The single-thread roles (tcgen05.mma / commit issue, TMA bulk copies) must
-// be entered through THIS predicate, not `lane == 0`: the instructions take their operands from uniform registers, and
-// under a lane-id predicate the compiler cannot prove uniformity, so it wraps EVERY such instruction in an
-// ELECT / BRA.U.ANY loop -- measured at ~95 cycles per tcgen05.mma (csrc/microbench.cu) against 64 cycles of tensor
-// work for a 128 x 128 x 16 step, i.e. the issue loop, not the tensor core, paced every GEMM and the attention kernel.
+// One elected lane of a fully converged warp, for the single-thread roles (TMA bulk copies).  Under a plain `lane == 0`
+// predicate the compiler cannot prove uniformity of the operands those instructions take from uniform registers.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(pred));
@@ -288,96 +281,64 @@ __device__ __forceinline__ bool elect_one() {
 }
 
 // ------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (warpgroup MMA): 64 x N x 16 per warpgroup, fp16 operands, fp32 accumulators in registers
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]^T, 16-bit float operands (format in the instruction descriptor), fp32 accumulate, cta_group::1
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// all previously issued MMAs of this thread arrive on `bar` when complete
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread i of the warp gets lane (base_lane + i), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ uint32_t tmem_ld1(uint32_t taddr) {      // one column: thread i gets lane (base_lane + i)
-  uint32_t r;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(taddr) : "memory");
-  return r;
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-// Accumulator read of the GEMM: the tile lives in TMEM as two column blocks DIST apart -- [A W_hi^T (+ A_lo W_hi^T) | A W_lo^T],
-// written by ONE N = 2 BN tcgen05.mma per K step (gemm.cu) -- and the value is their sum.  The second block is read in two
-// 16-column pieces so that at most 48 registers are live.  Includes the tcgen05.wait::ld.
-template <int DIST, bool STACKED>
-__device__ __forceinline__ void acc_ld32(uint32_t taddr, uint32_t* r) {
-  if (!STACKED) {
-    tmem_ld32(taddr, r);
-    tmem_ld_wait();
-    return;
-  }
-  uint32_t t[16];
-  tmem_ld32(taddr, r);
-  tmem_ld16(taddr + DIST, t);
-  tmem_ld_wait();
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// The accumulator registers are read and written by the asynchronous MMA: this keeps the compiler from moving
+// their uses across wgmma_commit / wgmma_wait.
+template <int NR>
+__device__ __forceinline__ void wgmma_fence_regs(float* d) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) + __uint_as_float(t[i]));
-  tmem_ld16(taddr + DIST + 16, t);
-  tmem_ld_wait();
-#pragma unroll
-  for (int i = 0; i < 16; ++i) r[16 + i] = __float_as_uint(__uint_as_float(r[16 + i]) + __uint_as_float(t[i]));
+  for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// K-major, 128-byte-swizzled operand tile descriptor (rows of 128 B, 8-row groups 1024 B apart).
-// Field layout: cute/arch/mma_sm100_desc.hpp (SmemDescriptor): start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout SWIZZLE_128B=2 [61,64).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  return static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 46) |
-         (2ull << 61);
+// K-major, 128-byte-swizzled operand tile descriptor (rows of 128 B, 8-row groups 1024 B apart; tile base 1024-aligned).
+// Field layout (PTX ISA, "Matrix Descriptor Format" of wgmma): start>>4 [0,14), LBO>>4 [16,30) (unused for swizzled
+// K-major: 1), SBO>>4 [32,46) = 1024 B, layout type [62,64) with SWIZZLE_128B = 1.  +2 on the descriptor = next 16 fp16 of K.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+  return static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// Instruction descriptor (InstrDescriptor): c_format F32=1 [4,6), a/b_format F16=0 [7,10)/[10,13) (BF16 would be 1),
-// a/b major K=0, n_dim = N>>3 [17,23), m_dim = M>>4 [24,29).
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t M, uint32_t N) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
+
+// D (+)= A[smem] * B[smem]^T, both K-major; scale_d == 0 overwrites D.  Accumulator fragment of thread (warp w of the
+// warpgroup, lane = 4 g + t): d[4 j + {0,1}] = row 16 w + g, columns 8 j + 2 t + {0,1}; d[4 j + {2,3}] = row + 8, same columns.
+template <int N>
+__device__ __forceinline__ void wgmma_ss(float* d, uint64_t da, uint64_t db, uint32_t scale_d);
+template <>
+__device__ __forceinline__ void wgmma_ss<32>(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <>
+__device__ __forceinline__ void wgmma_ss<64>(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <>
+__device__ __forceinline__ void wgmma_ss<128>(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <int N>
+__device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d);
+template <>
+__device__ __forceinline__ void wgmma_rs<32>(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
 }
 
 }  // namespace aldm

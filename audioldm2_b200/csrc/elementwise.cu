@@ -117,7 +117,7 @@ extern "C" int aldm_ddim_step(const float* x, const float* eps_uncond, const flo
   c.g = guidance;
   const long long n4 = n_total / 4;
   long long blocks = (n4 + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > num_sms() * 8) blocks = num_sms() * 8;
   ddim_step_kernel<<<(unsigned)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const float4*>(x), reinterpret_cast<const float4*>(eps_uncond),
       reinterpret_cast<const float4*>(eps_cond), reinterpret_cast<const float4*>(noise),

@@ -1,24 +1,22 @@
-// K1/K2/K7/K8: implicit-GEMM convolution / linear layer on tcgen05 tensor cores.
+// K1/K2/K7/K8: implicit-GEMM convolution / linear layer on Hopper tensor cores (wgmma).
 //
 //   out[row(m), n] = epilogue( sum_k A[m,k] * W[n,k] )        (aldm_gemm_desc, include/aldm_b200.h)
 //
-// Precision: split-fp16 operands, fp32 accumulation in TMEM.  Weights are packed as two fp16 planes (w ~= hi + lo,
+// Precision: split-fp16 operands, fp32 accumulation in registers.  Weights are packed as two fp16 planes (w ~= hi + lo,
 // 22 significand bits).  Activations arrive as fp16 planes written by the prep kernels / producer epilogues:
-//   * two planes (a_lo != NULL): the products hi*hi + hi*lo_w + lo*hi_w, ~2^-22 operand precision, issued as TWO kind::f16
-//     instructions per K step (A_hi against the stage's [W_hi ; W_lo] as one N = 2 BN operand, A_lo against W_hi) -- the
-//     convolutions, where the 200-step waveform budget goes (DESIGN.md section 3, scripts/precision_study.py);
-//   * one plane (a_lo == NULL): two instructions (hi*lo_w, hi*hi_w) and half the A bytes -- the token-side linear layers.
+//   * two planes (a_lo != NULL): the products hi*hi + hi*lo_w + lo*hi_w, ~2^-22 operand precision, three wgmma per
+//     K step -- the convolutions, where the 200-step waveform budget goes (DESIGN.md section 3, scripts/precision_study.py);
+//   * one plane (a_lo == NULL): two wgmma (hi*lo_w, hi*hi_w) and half the A bytes -- the token-side linear layers.
 // (SURVEY.md 7 H1: plain single-pass bf16 / TF32-class rounding of BOTH operands misses or crowds the 1e-3 waveform
 // tolerance; rounding only the activations to 11 bits costs 2e-4 at 200 steps.)
 //
-// Structure of one CTA (persistent: 448 threads, one CTA per SM looping over 128 x BN output tiles / split-K slices; details
-// and the measurements behind them at gemm_tc3_kernel below and in DESIGN.md section 4):
-//   warps 0-3   A producers: gather 16-byte chunks (8 channels of one tap of one pixel) with cp.async + zero fill into
+// Structure of one CTA (persistent: 416 threads, one CTA per SM looping over 128 x BN output tiles / split-K slices):
+//   warps 0-7   two consumer warpgroups: wgmma on 64-row halves of the tile, then the epilogue of the tile from an fp32
+//               copy of the accumulator in shared memory.
+//   warps 8-11  A producers: gather 16-byte chunks (8 channels of one tap of one pixel) with cp.async + zero fill into
 //               128B-swizzled K-major tiles; completion is signalled on the stage's mbarrier (cp.async.mbarrier.arrive).
-//   warp 4      B producer: one ELECTED lane (elect.sync) issues a TMA bulk copy (cp.async.bulk) of the host-packed,
+//   warp 12     B producer: one ELECTED lane (elect.sync) issues a TMA bulk copy (cp.async.bulk) of the host-packed,
 //               pre-swizzled weight tile image (hi|lo) per stage.
-//   warp 5      allocates TMEM; one elected lane issues tcgen05.mma into a double-buffered accumulator and commits stages.
-//   warps 6-13  epilogue out of TMEM, overlapping the next tile's main loop.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -167,7 +165,7 @@ __device__ __forceinline__ CoRows co_rows(const RowInfo& r, int lane) {
   return cr;
 }
 
-// issue the residual loads of one 32-column chunk (they are consumed after the TMEM read + transpose,
+// issue the residual loads of one 32-column chunk (they are consumed after the accumulator read + transpose,
 // and the next chunk's loads are issued before the current chunk is processed: latency hidden)
 __device__ __forceinline__ void co_load_res(const aldm_gemm_desc& d, const CoRows& cr, int n0, int n_out, int lane, float4 (&rv)[8]) {
   const int rs = lane >> 3, n = n0 + (lane & 7) * 4;
@@ -283,8 +281,8 @@ __device__ __forceinline__ void emit_rows(const aldm_gemm_desc& d, const CR& cr,
 
 // ---- full-line finish for single-plane fp16 outputs (EPI_PLN, EPI_GEGLU -> planes) ------------------------
 // A warp's 32 x 32 chunk is only 64 bytes per row in fp16: stored by itself it is a stream of half-line transactions, and the
-// SM's store port moves one transaction per clock whatever its size (32 B/clk for full lines: profiles/r02_store_port_rate.txt;
-// the GEGLU epilogue spent 2,500 of its 5,100 cycles per tile storing 16 KB).  The two warps that own the same TMEM lane quarter
+// SM's store port moves one transaction per clock whatever its size (scripts/store_rate.py measures it), so half-line
+// stores halve the store bandwidth of the epilogue.  The two warps that own the same accumulator row quarter
 // (chunk parity 0 / 1: columns [0,32) and [32,64) of one 64-column group) therefore assemble the 32 x 64 fp16 block in a shared
 // tile (rows of 128 bytes, 16-byte chunks XOR-swizzled by the row), meet at a 64-thread named barrier, and each stores 16
 // complete 128-byte rows: 4 STG.128 per warp instead of 8 STG.64.  Two tiles alternate, so one barrier per block suffices.
@@ -318,20 +316,42 @@ struct Tc3Cfg {
   static constexpr int B_BYTES = BN * 128;            // one plane
   static constexpr int STAGE_BYTES = AP * A_BYTES + 2 * B_BYTES;      // [a_hi | a_lo (AP == 2)] [b_hi | b_lo]
   static constexpr int B_OFF = AP * A_BYTES;
+  static constexpr int ACC_BYTES = BM * BN * 4;       // fp32 accumulator tile handed from the warpgroups to the epilogue
   static constexpr int STG_BYTES = 8 * 32 * 33 * 4;   // one 32x33 fp32 transpose tile per epilogue warp
   static constexpr int SMEM_MAX = 227 * 1024;
-  static constexpr int FIT = (SMEM_MAX - 1024 - 256 - STG_BYTES) / STAGE_BYTES;
-  static constexpr int STAGES = FIT > 4 ? 4 : FIT;    // BN=128: 3 (AP=2, 64 KB stages) / 4 (AP=1, 48 KB)
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + STG_BYTES;
-  // ST ("stacked"): the B stage [W_hi rows | W_lo rows] is issued as ONE N = 2 BN operand, so the accumulator is two column
-  // blocks [A W_hi^T (+ A_lo W_hi^T) | A W_lo^T] that the epilogue adds.  Used for the two-plane (convolution) operands, whose
-  // long K loops are tensor-bound: 2 instead of 3 instructions per K step (measured 273 vs 314 cycles, csrc/microbench.cu).  The
-  // single-plane token-side GEMMs keep the plain form: their short K loops are epilogue-bound and the second TMEM read of the
-  // stacked form made them slower (lin_k256_n768_qkv 34.6 -> 44.6 us), while their MMA time hides under the epilogue anyway.
-  static constexpr bool ST = AP == 2;
-  static constexpr int TMEM_COLS = ST ? 2 * BN : BN;  // one accumulator (power of two >= 32)
+  static constexpr int FIT = (SMEM_MAX - 1024 - 256 - STG_BYTES - ACC_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = FIT > 4 ? 4 : FIT;    // BN=128: 2 stages; BN=64: 3; BN=32: 4
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + STG_BYTES;
   static_assert(STAGES >= 2, "pipeline needs two stages");
+  static_assert(SMEM_BYTES <= SMEM_MAX, "shared memory");
 };
+
+// Accumulator tile in shared memory: row-major fp32 [BM][BN], the 16-byte chunk index XOR-swizzled by (row & 7), so that
+// the wgmma fragment stores and the row-per-lane reads of the epilogue (acc_ld32) are both free of bank conflicts.
+template <int BN>
+__device__ __forceinline__ void acc_st_frag(float* accb, int row0, int lane, const float* d) {
+  const int g = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + g + 8 * h;
+    float* rp = accb + row * BN + 2 * (t & 1);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+      *reinterpret_cast<float2*>(rp + (((2 * j + (t >> 1)) ^ (row & 7)) << 2)) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+  }
+}
+// columns [c0, c0 + 32) of accumulator row `row`
+template <int BN>
+__device__ __forceinline__ void acc_ld32(const float* accb, int row, int c0, uint32_t* r) {
+  const float* rp = accb + row * BN;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float4 x = *reinterpret_cast<const float4*>(rp + ((((c0 >> 2) + j) ^ (row & 7)) << 2));
+    r[4 * j] = __float_as_uint(x.x); r[4 * j + 1] = __float_as_uint(x.y);
+    r[4 * j + 2] = __float_as_uint(x.z); r[4 * j + 3] = __float_as_uint(x.w);
+  }
+}
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // Debug timeline (profiling aid, dbg bit 128): CTA 0 records clock64() at pipeline events.
 // layout: [role 0..3][iteration 0..255][phase 0..1]
@@ -342,20 +362,15 @@ __device__ long long g_timeline[4 * 256 * 2];
   } while (0)
 
 // ------------------------------------------------------------------------------------------
-// persistent variant (default): one CTA per SM loops over output tiles; 448 threads =
-//   warps 0-3 A producers | warp 4 B (TMA bulk) | warp 5 MMA | warps 6-13 epilogue (two per TMEM lane
-//   quarter, alternating 32-column chunks).
-// Two TMEM accumulators (2 x BN columns) let the epilogue of tile i drain while the producers and the
-// tensor core already work on tile i+1; barrier init / TMEM alloc are paid once per CTA.
-// What the measured timeline (profiles/r01_gemm_timeline.txt) showed and this version fixes:
-//   * each role runs ONE warp per SM sub-partition, so dependent-instruction latency is fully exposed:
-//     the producers' per-stage address arithmetic (an integer division and eight 64-bit index chains)
-//     took ~1450 cycles against 768 cycles of MMA work.  Row bases and per-row tap-validity masks are
-//     now computed once per tile; a stage costs one add + one bit test per row.
-//   * the epilogue took ~26k cycles per tile with four warps and a generic (all modes inlined, 200 KB
-//     of SASS) body.  EPI selects a specialised body at compile time (0: linear/conv with optional
-//     bias, row vector, residual, dual/QKV plane outputs; 1: GEGLU; 2: everything else), and eight
-//     warps share the drain.
+// persistent variant (default): one CTA per SM loops over output tiles; 416 threads =
+//   warps 0-7 two consumer warpgroups (wgmma into register accumulators, rows [64 wg, 64 wg + 64) of the tile),
+//   then the epilogue of the same tile | warps 8-11 A producers | warp 12 B (TMA bulk).
+// The finished accumulator is staged in shared memory (fp32, 16-byte chunks swizzled by row) so that each epilogue
+// warp reads whole rows: warp ew owns rows [32 (ew & 3), +32) and alternates 32-column chunks with warp ew ^ 4.
+// While the consumers run the epilogue, the producers already fill the pipeline with the next tile's stages.
+// The producers' per-stage work is one add + one bit test per row: row bases and per-row tap-validity masks are
+// computed once per tile.  EPI selects a specialised epilogue body at compile time (0: linear/conv with optional
+// bias, row vector, residual, dual/QKV plane outputs; 1: GEGLU; 2: everything else; 3/4: compact fp32 / planes).
 // Tile order: split-K slice fastest, then n-tile, then m-tile, so CTAs running concurrently share the
 // same activation rows in L2.
 // ------------------------------------------------------------------------------------------
@@ -388,21 +403,19 @@ struct Tc3Divs {
   int plain;      // 1x1 tap, unit stride, no upsample / batch-modulo: input row == output row (linear layers)
 };
 
-// AP = number of A planes (2: hi + lo, three UMMAs per K step; 1: hi only, two UMMAs and half the A bytes).
+// AP = number of A planes (2: hi + lo, three MMAs per K step; 1: hi only, two MMAs and half the A bytes).
 template <int BN, int EPI, int AP>
-__global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant__ aldm_gemm_desc d, int tiles_m, int tiles_n,
+__global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant__ aldm_gemm_desc d, int tiles_m, int tiles_n,
                                                            const __grid_constant__ Tc3Divs fd) {
   using C = Tc3Cfg<BN, AP>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
-  const uint32_t bar_base = base + C::STAGES * C::STAGE_BYTES;
+  const uint32_t acc_base = base + C::STAGES * C::STAGE_BYTES;
+  const uint32_t bar_base = acc_base + C::ACC_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * C::STAGES + 4);
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - raw));
+  float* accb = reinterpret_cast<float*>(smem_raw + (acc_base - raw));
 
   const int tid = threadIdx.x;
   const int warp = tid >> 5;
@@ -415,26 +428,15 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
   if (tid == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(full_bar(s), 128 + 1);   // 128 cp.async producers (completion-triggered arrivals) + B expect_tx
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);        // tcgen05.commit after the tile's last k-block
-      mbar_init(tempty_bar(a), 8);       // one arrival per epilogue warp
+      mbar_init(empty_bar(s), 8);        // one arrival per consumer warp once its MMAs on the stage have completed
     }
     fence_barrier_init();
   }
-  if (warp == 5) {
-    tmem_alloc(tmem_slot, 2 * C::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
   // Everything above overlapped the predecessor's tail; nothing below may touch its outputs before the wait.
-  // The weight stream is the exception (ALDM_GEMM_STATIC_B): warp 4 starts filling the pipeline right away.
+  // The weight stream is the exception (ALDM_GEMM_STATIC_B): warp 12 starts filling the pipeline right away.
   // The A producers wait inside their branch, after the (memory-free) row decode of their first tile.
-  if (warp > 4 || (warp == 4 && !(d.impl & ALDM_GEMM_STATIC_B))) pdl_wait();
+  if (warp < 8 || (warp == 12 && !(d.impl & ALDM_GEMM_STATIC_B))) pdl_wait();
 
   auto tile_coords = [&](int id, int& mt, int& nt, int& z, int& kb0, int& nkb) {
     int r = id;
@@ -448,10 +450,11 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
     fd.tn.divmod(r, mt, nt);
   };
 
-  if (warp < 4) {
+  if (warp >= 8 && warp < 12) {
     // ===================== A producers =====================
-    const int j = tid & 7;                 // 16-byte chunk (8 channels) inside the 64-wide K block
-    const int rbase = tid >> 3;            // rows rbase + 16*i
+    const int ptid = tid - 256;
+    const int j = ptid & 7;                 // 16-byte chunk (8 channels) inside the 64-wide K block
+    const int rbase = ptid >> 3;            // rows rbase + 16*i
     const uint32_t swz = (uint32_t)((j ^ (rbase & 7)) << 4);
     const int Hs = d.H >> d.up, Ws = d.W >> d.up;
     const aldm_plane_t* ahi = reinterpret_cast<const aldm_plane_t*>(d.a_hi);
@@ -461,10 +464,9 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
     int rowoff[8];            // element offset of tap (0,0) / channel 0 of each row (valid rows only)
     uint32_t tapmask[8];      // bit (t + 4) set <=> tap t of this row is inside the input (pre-shifted: (mask >> t) & 16 = bytes to copy)
     int ih0[8], iw0[8], pbh[8];   // only used by the nearest-upsample (up = 1) slow path
-    // Row decode of one M tile.  A single warp per scheduler runs this dependent integer chain at ~1 instruction
-    // per 6-8 cycles, and the timeline showed ~5,000 idle tensor-core cycles at every tile boundary of the K = 256
-    // linear layers because of it: linear layers take the trivial branch, and the first tile is decoded before the
-    // programmatic-dependency wait (under the previous kernel's tail).
+    // Row decode of one M tile.  A single warp per scheduler runs this dependent integer chain slowly and the tensor
+    // core idles meanwhile at every tile boundary of the short-K linear layers: linear layers take the trivial branch,
+    // and the first tile is decoded before the programmatic-dependency wait (under the previous kernel's tail).
     auto decode_rows = [&](int mt) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -514,15 +516,15 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
       for (int it = 0; it < nkb; ++it, ++cnt) {
         const int s = cnt % C::STAGES;
         mbar_wait(empty_bar(s), ((cnt / C::STAGES) & 1) ^ 1);
-        if (tid == 0) ALDM_TL(0, cnt, 0);
+        if (ptid == 0) ALDM_TL(0, cnt, 0);
         const bool kvalid = tap < d.ntaps;
         const int tp = kvalid ? tap : 0;
         const uint32_t sa = base + s * C::STAGE_BYTES + swz;
-        // Per 16-byte copy the producers now issue 3 (linear) / 4 (conv) instructions instead of ~9: the destination is one
-        // register + an immediate, the byte count (16 or 0 = zero fill) is a shift + mask of the per-row tap mask, and the
-        // source is one 64-bit add on a per-k-block base.  (The timeline showed the four producer warps -- one per scheduler,
-        // every dependent instruction fully exposed -- pacing the whole pipeline at ~710 cycles per k-block.)  A source
-        // address whose byte count is 0 is never dereferenced (cp.async zero-fill), so it needs no clamping.
+        // Per 16-byte copy the producers issue 3 (linear) / 4 (conv) instructions: the destination is one register + an
+        // immediate, the byte count (16 or 0 = zero fill) is a shift + mask of the per-row tap mask, and the source is one
+        // 64-bit add on a per-k-block base.  The four producer warps run one per scheduler with every dependent instruction
+        // exposed, so this count paces the pipeline.  A source address whose byte count is 0 is never dereferenced
+        // (cp.async zero-fill), so it needs no clamping.
         if (fd.plain) {
           const uint32_t kb = (kvalid && c < d.Cp) ? 16u : 0u;
           const aldm_plane_t* ab = ahi + (kb ? c : 0);
@@ -567,12 +569,12 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
           }
         }
         cp_async_mbar_arrive_noinc(full_bar(s));
-        if (tid == 0) ALDM_TL(0, cnt, 1);
+        if (ptid == 0) ALDM_TL(0, cnt, 1);
         c += C::BK;
         while (c >= d.Cp) { c -= d.Cp; ++tap; }
       }
     }
-  } else if (warp == 4) {
+  } else if (warp == 12) {
     // ===================== B producer =====================
     if (elect_one()) {
       uint32_t cnt = 0;
@@ -592,62 +594,52 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
       }
     }
     __syncwarp();
-  } else if (warp == 5) {
-    // ===================== MMA issuer =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_f16(128, BN), idesc2 = umma_idesc_f16(128, 2 * BN);
-      uint32_t cnt = 0, tl = 0;
-      for (int id = blockIdx.x; id < total; id += gridDim.x, ++tl) {
-        int mt, nt, z, kb0, nkb;
-        tile_coords(id, mt, nt, z, kb0, nkb);
-        const uint32_t acc = tl & 1;
-        mbar_wait(tempty_bar(acc), ((tl >> 1) & 1) ^ 1);      // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + acc * C::TMEM_COLS;
-        for (int it = 0; it < nkb; ++it, ++cnt) {
-          const int s = cnt % C::STAGES;
-          mbar_wait(full_bar(s), (cnt / C::STAGES) & 1);
-          ALDM_TL(2, cnt, 0);
-          tc_fence_after();
-          const uint32_t sa = base + s * C::STAGE_BYTES;
-          const uint64_t da_hi = umma_desc_sw128(sa);
-          const uint64_t da_lo = umma_desc_sw128(sa + C::A_BYTES);      // only used when AP == 2
-          const uint64_t db_hi = umma_desc_sw128(sa + C::B_OFF);
-          const uint64_t db_lo = umma_desc_sw128(sa + C::B_OFF + C::B_BYTES);      // only used by the plain (not stacked) form
-          if (!(dbg & 4)) {
-            // Measured (csrc/microbench.cu): a shared-memory-operand tcgen05.mma costs ~42 cycles + N / 2 -- the A fetch is
-            // not overlapped -- so one N = 256 instruction (169 cycles) is cheaper than two N = 128 ones (2 x 105).
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {            // 4 x K=16 (32 bytes) inside the 128B swizzle row
-              const uint64_t o = (uint64_t)(ks * 2);
-              if (C::ST) {
-                umma_f16(tacc, da_hi + o, db_hi + o, idesc2, (uint32_t)((it | ks) != 0));      // [A_hi W_hi^T | A_hi W_lo^T]
-                umma_f16(tacc, da_lo + o, db_hi + o, idesc, 1);                                // + A_lo W_hi^T into the first block
-              } else {
-                umma_f16(tacc, da_hi + o, db_lo + o, idesc, (uint32_t)((it | ks) != 0));       // small term first
-                umma_f16(tacc, da_hi + o, db_hi + o, idesc, 1);
-              }
-            }
-          }
-          umma_commit(empty_bar(s));
-          ALDM_TL(2, cnt, 1);
-        }
-        umma_commit(tfull_bar(acc));
-      }
-      pdl_launch();     // all MMAs of this CTA are issued: let the next kernel's blocks be scheduled under the last epilogue
-    }
-    __syncwarp();
   } else {
-    // ===================== epilogue: warps 6-13; TMEM lane quarter = warp % 4, chunk parity = (warp-6)/4 =====================
-    const int lb = warp & 3;
-    const int half = (warp - 6) >> 2;
+    // ===================== consumers: warpgroup wg = rows [64 wg, 64 wg + 64) of the tile; then the epilogue =====================
+    const int wg = warp >> 2;
+    const int ew = warp;                 // epilogue role: rows [32 lb, 32 lb + 32), chunk parity `half`
+    const int lb = ew & 3;
+    const int half = ew >> 2;
     const int trow_in_tile = lb * 32 + lane;
-    float* stg = reinterpret_cast<float*>(smem_raw + (bar_base + 256 - raw)) + (warp - 6) * (32 * 33);
-    uint32_t tl = 0, pair_cnt = 0;
+    float* stg = reinterpret_cast<float*>(smem_raw + (bar_base + 256 - raw)) + ew * (32 * 33);
+    uint32_t cnt = 0, tl = 0, pair_cnt = 0;
+    float acc[BN / 2];
     for (int id = blockIdx.x; id < total; id += gridDim.x, ++tl) {
       int mt, nt, z, kb0, nkb;
       tile_coords(id, mt, nt, z, kb0, nkb);
-      const uint32_t acc = tl & 1;
+      // (the asm operands are read-write: a defined start value keeps the accumulator dead during the epilogue)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int it = 0; it < nkb; ++it, ++cnt) {
+        const int s = cnt % C::STAGES;
+        mbar_wait(full_bar(s), (cnt / C::STAGES) & 1);
+        if (tid == 0) ALDM_TL(2, cnt, 0);
+        fence_proxy_async();          // cp.async-written A tiles -> visible to the tensor core (async proxy)
+        const uint32_t sa = base + s * C::STAGE_BYTES;
+        const uint64_t da_hi = wgmma_desc_sw128(sa + wg * 64 * 128);
+        const uint64_t da_lo = wgmma_desc_sw128(sa + C::A_BYTES + wg * 64 * 128);      // only used when AP == 2
+        const uint64_t db_hi = wgmma_desc_sw128(sa + C::B_OFF);
+        const uint64_t db_lo = wgmma_desc_sw128(sa + C::B_OFF + C::B_BYTES);
+        wgmma_fence();
+        if (!(dbg & 4)) {
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) {            // 4 x K=16 (32 bytes) inside the 128B swizzle row
+            const uint64_t o = (uint64_t)(ks * 2);
+            wgmma_ss<BN>(acc, da_hi + o, db_lo + o, 1);      // small terms first
+            if (AP == 2) wgmma_ss<BN>(acc, da_lo + o, db_hi + o, 1);
+            wgmma_ss<BN>(acc, da_hi + o, db_hi + o, 1);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();              // the previous stage's MMAs have completed: release it
+        if (it > 0 && lane == 0) mbar_arrive(empty_bar((cnt - 1) % C::STAGES));
+        if (tid == 0) ALDM_TL(2, cnt, 1);
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs<BN / 2>(acc);
+      if (lane == 0) mbar_arrive(empty_bar((cnt - 1) % C::STAGES));
+      // all MMAs of this CTA are done: let the next kernel's blocks be scheduled under the last epilogue
+      if (tid == 0 && id + (int)gridDim.x >= total) pdl_launch();
       const int m = mt * C::BM + trow_in_tile;
       RowInfo r;
       {
@@ -674,9 +666,8 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
           const int n = nt * BN + half * 32 + 64 * ch + (lane & 7) * 4;
           pb4[ch] = (d.bias && n < d.N) ? __ldg(reinterpret_cast<const float4*>(d.bias + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
-        // BOTH chunks' residuals are requested here, under the accumulator wait: issued after the first chunk was staged (the
-        // previous version) the loads queued behind the chunk's stores in the LSU -- 1,000-2,000 cycles from "staged" to
-        // "loads issued" in the timeline -- and the second chunk then waited for them.
+        // BOTH chunks' residuals are requested here, before the accumulator is staged: issued after the first chunk was
+        // staged, the loads would queue behind that chunk's stores in the LSU and the second chunk would wait for them.
 #pragma unroll
         for (int ch = 0; ch < NRV; ++ch)
           if (has_res && half * 32 + 64 * ch < BN) co_load_res32(d, cr32, nt * BN + half * 32 + 64 * ch, d.N, lane, prv[ch]);
@@ -688,8 +679,8 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
                               (d.N / 2) % 64 == 0 && d.ldo % 8 == 0 && (reinterpret_cast<uintptr_t>(d.out_hi) & 15u) == 0;
       const bool pair_qk = EPI == EPI_FAST && BN >= 64 && d.out_mode == ALDM_OUT_QKV && d.out_lo == nullptr && d.res == nullptr &&
                            d.splitk == 1 && d.n_split % 64 == 0 && d.ldo % 8 == 0 && (reinterpret_cast<uintptr_t>(d.out_hi) & 15u) == 0;
-      uint8_t* pair_tiles = reinterpret_cast<uint8_t*>(smem_raw + (bar_base + 256 - raw)) + ((warp - 6) & 3) * (32 * 33 * 4);
-      const int pair_bar = 1 + ((warp - 6) & 3);
+      uint8_t* pair_tiles = reinterpret_cast<uint8_t*>(smem_raw + (bar_base + 256 - raw)) + (ew & 3) * (32 * 33 * 4);
+      const int pair_bar = 1 + (ew & 3);
       float pln_b[NCH > 0 ? NCH : 1];      // bias of this warp's columns (lane = column), distributed by shuffles in pair mode
 #pragma unroll
       for (int ch = 0; ch < NCH; ++ch) {
@@ -701,11 +692,12 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
         gb_v = __ldg(d.bias + nt * BN + half * 32 + lane);
         gb_g = __ldg(d.bias + nt * BN + BN / 2 + half * 32 + lane);
       }
-      if (warp == 6 && lane == 0) ALDM_TL(3, 64 + tl * 8, 0);      // tile prologue (row decode, bias / residual prefetch) done
-      mbar_wait(tfull_bar(acc), (tl >> 1) & 1);
-      if (warp == 6 && lane == 0) ALDM_TL(3, tl, 0);
-      tc_fence_after();
-      const uint32_t trow = tmem_base + acc * C::TMEM_COLS + ((uint32_t)(lb * 32) << 16);
+      if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8, 0);      // tile prologue (row decode, bias / residual prefetch) done
+      // stage the accumulator tile in shared memory, once every warp is done reading the previous tile's
+      named_bar_sync(5, 256);
+      acc_st_frag<BN>(accb, wg * 64 + (warp & 3) * 16, lane, acc);
+      named_bar_sync(5, 256);
+      if (ew == 0 && lane == 0) ALDM_TL(3, tl, 0);
       if (dbg & 8) {
         // skip
       } else if (d.splitk > 1) {
@@ -715,7 +707,7 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
 #pragma unroll 1
         for (int c0 = half * 32; c0 < BN; c0 += 64) {
           uint32_t v[32];
-          acc_ld32<BN, C::ST>(trow + c0, v);
+          acc_ld32<BN>(accb, trow_in_tile, c0, v);
 #pragma unroll
           for (int i = 0; i < 32; ++i) stg[lane * 33 + i] = __uint_as_float(v[i]);
           __syncwarp();
@@ -738,13 +730,13 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
         for (int c0 = half * 32; c0 < BN / 2; c0 += 64) {
           const int n0 = nt * (BN / 2) + c0;
           uint32_t vr[32], gr[32];
-          acc_ld32<BN, C::ST>(trow + c0, vr);
-          acc_ld32<BN, C::ST>(trow + BN / 2 + c0, gr);
-          if (warp == 6 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1, 0);
+          acc_ld32<BN>(accb, trow_in_tile, c0, vr);
+          acc_ld32<BN>(accb, trow_in_tile, BN / 2 + c0, gr);
+          if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1, 0);
           float* v = reinterpret_cast<float*>(vr);
           float* g = reinterpret_cast<float*>(gr);
           // bias: fetched (one coalesced load per warp) BEFORE the accumulator wait, distributed by shuffles -- the broadcast
-          // float4 loads it replaces sat between the TMEM read and the GELU with a full L2 round trip exposed
+          // float4 loads it replaces sat between the accumulator read and the GELU with a full L2 round trip exposed
 #pragma unroll
           for (int i = 0; i < 32; ++i) {
             v[i] += __shfl_sync(0xffffffffu, gb_v, i);
@@ -752,15 +744,15 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
           }
 #pragma unroll      // full unroll: v/g must stay in registers (a partial unroll indexes them dynamically -> local memory)
           for (int i = 0; i < 32; i += 8) geglu_mul<8>(v + i, g + i);
-          if (warp == 6 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1, 1);
+          if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1, 1);
           if (pair_geglu) {                         // the FF1 case: one fp16 plane for FF2, stored as full lines by the warp pair
             emit_pair_hi(d, cr, nt * (BN / 2), pair_tiles + ((pair_cnt++ & 1u) ? 4 * (32 * 33 * 4) : 0), lane, half, pair_bar, v);
-            if (warp == 6 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2, 1);
+            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2, 1);
           } else if (d.out_mode == ALDM_OUT_PLANES) {
             stage_rows(stg8, lane, v);
-            if (warp == 6 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2, 0);
+            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2, 0);
             emit_rows<true>(d, cr, n0, n_out, stg8, lane, rv, false, make_float4(0.f, 0.f, 0.f, 0.f));
-            if (warp == 6 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2, 1);
+            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2, 1);
           } else {
             epi_finish_coalesced(d, cr, n0, v, n_out, stg, lane, rv, false);
           }
@@ -770,7 +762,7 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
         for (int ch = 0; ch < NCH; ++ch) {
           const int c0 = half * 32 + 64 * ch;      // < BN: BN >= 64 in pair mode
           uint32_t vr[32];
-          acc_ld32<BN, C::ST>(trow + c0, vr);
+          acc_ld32<BN>(accb, trow_in_tile, c0, vr);
           float* v = reinterpret_cast<float*>(vr);
           if (d.bias) {
 #pragma unroll
@@ -785,13 +777,13 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
           if (c0 < BN) {
             const int n0 = nt * BN + c0;
             uint32_t vr[32];
-            acc_ld32<BN, C::ST>(trow + c0, vr);
-            if (warp == 6 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1 + 2 * ch, 0);
+            acc_ld32<BN>(accb, trow_in_tile, c0, vr);
+            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1 + 2 * ch, 0);
             stage_rows(stg8, lane, reinterpret_cast<const float*>(vr));
-            if (warp == 6 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1 + 2 * ch, 1);
-            if (warp == 6 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2 + 2 * ch, 0);
+            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1 + 2 * ch, 1);
+            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2 + 2 * ch, 0);
             emit_rows<EPI == EPI_PLN>(d, cr32, n0, d.N, stg8, lane, prv[ch % NRV], has_res, pb4[ch]);
-            if (warp == 6 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2 + 2 * ch, 1);
+            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2 + 2 * ch, 1);
           }
         }
       } else if (EPI == EPI_FAST) {
@@ -804,7 +796,7 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
           const bool pre = d.res != nullptr && !vpart;
           if (pre) co_load_res(d, cr, n0, d.N, lane, rv);
           uint32_t vr[32];
-          acc_ld32<BN, C::ST>(trow + c0, vr);
+          acc_ld32<BN>(accb, trow_in_tile, c0, vr);
           float* v = reinterpret_cast<float*>(vr);
           if (d.bias) add_vec32(v, d.bias + n0);
           if (d.rowvec) add_vec32(v, d.rowvec + (long long)r.b * d.ld_rowvec + n0);
@@ -837,29 +829,19 @@ __global__ void __launch_bounds__(448, 1) gemm_tc3_kernel(const __grid_constant_
           if (d.act == ALDM_ACT_GEGLU) {
             if (c0 >= BN / 2) break;
             uint32_t vr[32], gr[32];
-            acc_ld32<BN, C::ST>(trow + c0, vr);
-            acc_ld32<BN, C::ST>(trow + BN / 2 + c0, gr);
+            acc_ld32<BN>(accb, trow_in_tile, c0, vr);
+            acc_ld32<BN>(accb, trow_in_tile, BN / 2 + c0, gr);
             epi_activate(d, r, nt * BN + c0, reinterpret_cast<float*>(vr), reinterpret_cast<float*>(gr));
             epi_finish(d, r, nt * (BN / 2) + c0, 32, reinterpret_cast<float*>(vr), d.N / 2);
           } else {
             uint32_t vr[32];
-            acc_ld32<BN, C::ST>(trow + c0, vr);
+            acc_ld32<BN>(accb, trow_in_tile, c0, vr);
             epi_activate(d, r, nt * BN + c0, reinterpret_cast<float*>(vr), nullptr);
             epi_finish(d, r, nt * BN + c0, 32, reinterpret_cast<float*>(vr), d.N);
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-      if (warp == 6 && lane == 0) ALDM_TL(3, tl, 1);
     }
-  }
-
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 2 * C::TMEM_COLS);
   }
 }
 
@@ -909,8 +891,8 @@ __global__ void splitk_epilogue_kernel(const __grid_constant__ aldm_gemm_desc d,
 
 // Coalesced variant for the cases the planner actually splits (no activation, alpha = 1, no accumulate; fp32,
 // planes or dual output; bias / row vector / residual): one thread per (row, 4 columns), so the partial sums,
-// the residual and the outputs are all full-line float4 streams.  The row-owner kernel above took 22 us per
-// launch in the step's launch list (34 launches per DDIM step) for a few MB of traffic.
+// the residual and the outputs are all full-line float4 streams, where the row-owner kernel above issues scattered
+// per-row accesses for a few MB of traffic.
 __global__ void __launch_bounds__(256) splitk_reduce4_kernel(const __grid_constant__ aldm_gemm_desc d, int Mpad, int Npad) {
   pdl_wait();
   const int M = d.B * d.OH * d.OW;
@@ -1003,8 +985,6 @@ __global__ void gemm_simt_kernel(const __grid_constant__ aldm_gemm_desc d, int N
 // ------------------------------------------------------------------------------------------
 // host launch
 // ------------------------------------------------------------------------------------------
-static int g_num_sms = 0;
-
 template <int BN, int EPI, int AP>
 static int launch_tc3_ap(const aldm_gemm_desc& d, int M, cudaStream_t st) {
   using C = Tc3Cfg<BN, AP>;
@@ -1013,20 +993,15 @@ static int launch_tc3_ap(const aldm_gemm_desc& d, int M, cudaStream_t st) {
     ALDM_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc3_kernel<BN, EPI, AP>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     configured = true;
   }
-  if (g_num_sms == 0) {
-    int dev = 0;
-    ALDM_CHECK_CUDA(cudaGetDevice(&dev));
-    ALDM_CHECK_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev));
-  }
   const int tiles_m = cdiv(M, C::BM), tiles_n = cdiv(d.N, BN);
   const long long total = (long long)tiles_m * tiles_n * d.splitk;
-  const int grid = (int)(total < g_num_sms ? total : g_num_sms);
+  const int grid = (int)(total < num_sms() ? total : num_sms());
   Tc3Divs fd;
   fd.ow = make_fastdiv(d.OW); fd.oh = make_fastdiv(d.OH); fd.cp = make_fastdiv(d.Cp); fd.tn = make_fastdiv(tiles_n);
   fd.bmod = make_fastdiv(d.bmod > 0 ? d.bmod : 1);
   fd.plain = d.ntaps == 1 && d.dy[0] == 0 && d.dx[0] == 0 && d.sy == 1 && d.sx == 1 && d.up == 0 && d.bmod <= 0 &&
              d.OH == d.H && d.OW == d.W;
-  ALDM_CHECK_CUDA(launch_pdl(gemm_tc3_kernel<BN, EPI, AP>, dim3(grid), dim3(448), C::SMEM_BYTES, st, d, tiles_m, tiles_n, fd));
+  ALDM_CHECK_CUDA(launch_pdl(gemm_tc3_kernel<BN, EPI, AP>, dim3(grid), dim3(416), C::SMEM_BYTES, st, d, tiles_m, tiles_n, fd));
   ALDM_CHECK_CUDA(cudaGetLastError());
   if (d.splitk > 1) {
     const int Mpad = tiles_m * C::BM, Npad = tiles_n * BN;

@@ -1,107 +1,7 @@
-// Profiling aid (not on the product path): how fast does ONE SM retire tcgen05.mma instructions of a given shape when
-// nothing else touches shared memory?  scripts/umma_rate.py prints cycles per instruction for
-//   mode 0  SS: A and B from shared memory (what gemm_tc3_kernel issues), N in {32, 64, 128, 256}
-//   mode 1  TS: A from tensor memory, B from shared memory
-//   mode 2  SS with a concurrent shared-memory writer (cp.async-like generic stores from 4 warps) -- operand-port contention
-//   mode 3  TS with the A slice copied smem -> TMEM by tcgen05.cp (128x256b) right before each MMA: what a TS-mode GEMM would pay
-// The operands are whatever the shared / tensor memory holds (the values do not change the timing).
+// Profiling aid (not on the product path): SM -> L2 store throughput (scripts/store_rate.py).
 #include <stdlib.h>
 
 #include "common.cuh"
-
-namespace aldm {
-
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// smem -> TMEM copy of one 128 x 16 fp16 A slice (128 lanes x 256 bits), executed by the tensor pipe in issue order with the MMAs
-__device__ __forceinline__ void tmem_cp_128x256b(uint32_t tmem_dst, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.128x256b [%0], %1;" ::"r"(tmem_dst), "l"(sdesc) : "memory");
-}
-
-__global__ void __launch_bounds__(192, 1) umma_rate_kernel(int N, int mode, int reps, long long* out) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  const uint32_t a_sm = base, b_sm = base + 16384, bar = base + 16384 + 32768, slot = bar + 16;
-  const uint32_t scratch = bar + 1024;                      // 64 KB the writer warps scribble over (mode 2)
-  const int tid = threadIdx.x, warp = tid >> 5;
-  if (tid == 0) { mbar_init(bar, 1); fence_barrier_init(); }
-  if (warp == 5) { tmem_alloc(slot, 512); tmem_relinquish(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *reinterpret_cast<volatile uint32_t*>(smem_raw + (slot - raw));
-  __shared__ volatile int s_done;
-  if (tid == 0) s_done = 0;
-  __syncthreads();
-  auto issue = [&]() {
-    const uint32_t idesc = umma_idesc_f16(128, (uint32_t)N);
-    const uint64_t da = umma_desc_sw128(a_sm), db = umma_desc_sw128(b_sm);
-    const long long t0 = clock64();
-    for (int i = 0; i < reps; i += 4) {
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        const uint64_t o = (uint64_t)(ks * 2);
-        if ((mode & 3) == 1) {
-          umma_f16_ts(tmem, tmem + 256 + ks * 8, db + o, idesc, 1);
-        } else if ((mode & 3) == 3) {      // A staged smem -> TMEM by tcgen05.cp right before the MMA that reads it (two TMEM slots alternate)
-          tmem_cp_128x256b(tmem + 256 + ks * 8, da + o);
-          umma_f16_ts(tmem, tmem + 256 + ks * 8, db + o, idesc, 1);
-        } else {
-          umma_f16(tmem, da + o, db + o, idesc, 1);
-        }
-      }
-    }
-    umma_commit(bar);
-    mbar_wait(bar, 0);
-    const long long t1 = clock64();
-    out[blockIdx.x] = t1 - t0;
-    s_done = 1;
-  };
-  if (warp == 5) {
-    if (mode & 4) {           // mode bit 2: the issuing thread is chosen by elect.sync (the fix) instead of lane == 0
-      if (elect_one()) issue();
-    } else if ((tid & 31) == 0) {
-      issue();
-    }
-    __syncwarp();
-  } else if ((mode & 3) == 2 && warp < 4) {
-    // generic-proxy 16-byte stores, ~the rate the A producers + TMA write a stage (the values are never read)
-    uint32_t p = scratch + tid * 16;
-    int it = 0;
-    while (!s_done) {
-      asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};" ::"r"(p + (uint32_t)((it & 31) * 2048)), "r"(it) : "memory");
-      ++it;
-    }
-  }
-  __syncthreads();
-  if (warp == 5) { tc_fence_after(); tmem_dealloc(tmem, 512); }
-}
-
-}  // namespace aldm
-
-extern "C" int aldm_debug_umma_rate(int32_t N, int32_t mode, int32_t reps, long long* host_out, int32_t n_out) {
-  using namespace aldm;
-  ALDM_REQUIRE(host_out && n_out > 0 && reps > 0 && (N == 32 || N == 64 || N == 128 || N == 256) && mode >= 0 && mode <= 7, ALDM_E_ARG,
-               "debug_umma_rate: bad arguments");
-  long long* dev = nullptr;
-  ALDM_CHECK_CUDA(cudaMalloc(&dev, sizeof(long long) * n_out));
-  const int smem = 16384 + 32768 + 1024 + 65536 + 1024 + 1024;
-  ALDM_CHECK_CUDA(cudaFuncSetAttribute(umma_rate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  umma_rate_kernel<<<n_out, 192, smem>>>(N, mode, reps, dev);
-  ALDM_CHECK_CUDA(cudaGetLastError());
-  ALDM_CHECK_CUDA(cudaDeviceSynchronize());
-  ALDM_CHECK_CUDA(cudaMemcpy(host_out, dev, sizeof(long long) * n_out, cudaMemcpyDeviceToHost));
-  cudaFree(dev);
-  return ALDM_OK;
-}
 
 namespace aldm {
 

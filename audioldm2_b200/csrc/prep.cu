@@ -560,14 +560,14 @@ int prep_launch(const aldm_prep_desc& d, cudaStream_t st) {
       const GnGeom gg = gn_geom(C);
       const int thr = gg.QW * gg.RS;                 // multiple of 32 (Q is a multiple of 32 here), <= 256
       const int unit = 4 * gg.RS * cdiv(gg.Q, gg.QW);   // rows that give one thread four loads per column pass
-      int nblk = cdiv(4 * 148, d.B);
+      int nblk = cdiv(4 * num_sms(), d.B);
       if (nblk > cdiv(d.HW, 2 * unit)) nblk = cdiv(d.HW, 2 * unit);
       if (nblk > GN_MAX_BLOCKS) nblk = GN_MAX_BLOCKS;
       if (nblk < 1) nblk = 1;
       const int finalize = nblk > 8 ? 1 : 0;       // last-block finalisation only pays when the apply blocks would re-reduce many partials
       ALDM_CHECK_CUDA(launch_pdl(gn_stats_col_kernel, dim3(nblk, d.B), dim3(thr), 0, st, d, nblk, finalize));
       ALDM_CHECK_CUDA(cudaGetLastError());
-      int nap = cdiv(8 * 148, d.B);
+      int nap = cdiv(8 * num_sms(), d.B);
       if (nap > cdiv(d.HW, unit)) nap = cdiv(d.HW, unit);
       if (nap < 1) nap = 1;
       ALDM_CHECK_CUDA(launch_pdl(gn_apply_col_kernel, dim3(nap, d.B), dim3(thr), 0, st, d, finalize ? 0 : nblk));
@@ -585,7 +585,7 @@ int prep_launch(const aldm_prep_desc& d, cudaStream_t st) {
   } else if (d.mode == ALDM_PREP_LN) {
     ALDM_REQUIRE(d.gamma && d.beta, ALDM_E_ARG, "prep LN: null gamma/beta");
     ALDM_REQUIRE(d.c1 == 0 && C % 4 == 0 && C <= 1024 && d.Cp == C, ALDM_E_UNSUPPORTED, "prep LN: C=%d", C);
-    // one row per warp (NR = 2, two rows in flight per warp, measured SLOWER: 9.8 vs 8.2 us at 16384 x 256); float4 per lane sized to C
+    // one row per warp; float4 per lane sized to C
     const dim3 grid(cdiv(d.rows, 8));
     ALDM_CHECK_CUDA(C <= 256 ? launch_pdl(ln_kernel<2, 1>, grid, dim3(256), 0, st, d)
                              : (C <= 512 ? launch_pdl(ln_kernel<4, 1>, grid, dim3(256), 0, st, d) : launch_pdl(ln_kernel<8, 1>, grid, dim3(256), 0, st, d)));

@@ -21,6 +21,16 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
+int num_sms() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
+      n = 132;      // H100 SXM
+  }
+  return n;
+}
+
 bool pdl_enabled() {
   static const bool on = [] {
     const char* e = getenv("ALDM_PDL");
@@ -167,7 +177,7 @@ extern "C" const char* aldm_last_error(void) { return g_err; }
 extern "C" int aldm_device_check(int32_t device) {
   cudaDeviceProp prop;
   ALDM_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
-  ALDM_REQUIRE(prop.major == 10, ALDM_E_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_100a only", device,
+  ALDM_REQUIRE(prop.major == 9 && prop.minor == 0, ALDM_E_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device,
                prop.major, prop.minor);
   return ALDM_OK;
 }

@@ -29,7 +29,7 @@ class DeviceProgram:
     def __init__(self, plan: Plan, device: torch.device, ranges: Dict[str, Tuple[int, int]],
                  arena_dev: Optional[torch.Tensor] = None):
         if not torch.cuda.is_available():
-            raise RuntimeError("the native engine needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("the native engine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.L = _lib.lib()
         self.plan = plan
         self.device = torch.device(device)

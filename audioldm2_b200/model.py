@@ -89,10 +89,8 @@ def unpack_cond_dict(cond_dict: dict) -> dict:
 
 
 def default_lanes(batch: int) -> int:
-    """UNet lanes: 1 unless ALDM_LANES says otherwise.  Measured on the B200 (profiles/r02_sweep_lanes_switches.jsonl,
-    audioldm2-full, batch 8): 19.23 ms per DDIM step with one lane, 19.44 with two, 20.67 with four -- the parallel
-    branches do overlap (kernel count doubles at equal time) but what they hide at the deep levels is paid back in
-    split-K reductions, second weight streams and wave quantisation at the wide ones."""
+    """UNet lanes: 1 unless ALDM_LANES says otherwise.  Parallel lanes overlap the UNet's branches, but what they hide
+    at the deep levels is paid back in split-K reductions, second weight streams and wave quantisation at the wide ones."""
     env = os.environ.get("ALDM_LANES")
     if env:
         n = max(1, min(int(env), _lib.MAX_LANES))

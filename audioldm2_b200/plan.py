@@ -225,8 +225,11 @@ class Plan:
         return arr
 
 
+H100_SMS = 132      # SMs of the H100 SXM: the tile-count heuristics below size one wave of the persistent GEMM
+
+
 class Planner:
-    def __init__(self, impl: str = "tc", keep_plain: bool = False, splitk: bool = True, n_sm: int = 148):
+    def __init__(self, impl: str = "tc", keep_plain: bool = False, splitk: bool = True, n_sm: int = H100_SMS):
         self.impl = {"tc": _lib.GEMM_TC, "simt": _lib.GEMM_SIMT}[impl]
         self.keep_plain = keep_plain or impl == "simt"
         self.use_splitk = splitk and impl != "simt"
@@ -267,13 +270,11 @@ class Planner:
              bn: Optional[int] = None, m_rows: Optional[int] = None) -> WMat:
         N, K = wm.shape
         assert K == ntaps * cp
-        # Measured (profiles/r01_unet_ops_v4_eager.csv vs v5, and again in round 2: ALDM_NARROW=64 / 32 -> 16.3 / 17.5 ms per DDIM
-        # step against 16.1): narrower tiles as a general rule for small-M GEMMs are SLOWER (a second wave at the 256-pixel level,
-        # twice the weight traffic and no split-K for the long-K convolutions).  One case is different: a SHORT-K GEMM whose
-        # 128-wide tiles fill at most half the SMs (the 64-pixel level: 1024 x 640 x 640 = 40 tiles on 148 SMs) is a pure latency
-        # chain load -> MMA -> 64 KB of stores per CTA; halving the tile width halves the store phase (32 B/clk/SM store port,
-        # profiles/r02_store_port_rate.txt) and cuts the MMA time by 30 % (N = 64: 74 cycles per instruction against 105 for
-        # N = 128) while the tiles still fit one wave.  ALDM_HALF_TILES=0 switches it off (A/B).
+        # Narrower tiles as a general rule for small-M GEMMs cost a second wave at the 256-pixel level, twice the weight traffic
+        # and no split-K for the long-K convolutions (ALDM_NARROW=64 / 32 selects them, for experiments).  One case is different:
+        # a SHORT-K GEMM whose 128-wide tiles fill at most half the SMs (the 64-pixel level: 1024 x 640 x 640 = 40 tiles on 132
+        # SMs) is a latency chain load -> MMA -> 64 KB of stores per CTA; halving the tile width halves the MMA and store phases
+        # of each CTA while the tiles still fit one wave.  ALDM_HALF_TILES=0 switches it off (A/B).
         narrow = int(os.environ.get("ALDM_NARROW", "0"))       # experiment switch: smallest N tile the heuristic may pick
         explicit = bn is not None
         bn = bn or self.bn_for_rows(N, m_rows if narrow else None, geglu, min_bn=narrow or 32)
@@ -568,7 +569,7 @@ def build_unet(sd: Dict[str, torch.Tensor], cfg: dict, latent: Tuple[int, int, i
 
     def attention(nm: str, h: F32, norm: str, heads: int, Cc: int, HW: int, kv, mask: Optional[Ref]) -> F32:
         """x = attn(LN(x)) + x  (attention.py:343-367, 406-409).  The projection GEMMs write Q|K as operand
-        planes and V transposed (ALDM_OUT_QKV), which is what the tcgen05 attention kernel consumes."""
+        planes and V transposed (ALDM_OUT_QKV), which is what the wgmma attention kernel consumes."""
         p = P.prep(_lib.PREP_LN, h, None, P.vec(sd[norm + ".weight"]), P.vec(sd[norm + ".bias"]), eps=1e-5, n=TP)
         ao = P.planes(h.rows, Cc, TP)
         scale = (Cc // heads) ** -0.5

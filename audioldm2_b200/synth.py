@@ -1,6 +1,6 @@
 """Seeded synthetic checkpoints with the reference ``state_dict`` layout.
 
-There is no network on the build or GPU boxes, so hub checkpoints cannot be fetched
+Hub checkpoints cannot be assumed reachable (no network), so they are not fetched
 (utils.py:209-219).  Parity and throughput are therefore measured on deterministic
 random weights that have exactly the key names / shapes of the reference modules
 (SURVEY.md 8b/8d).  Rules (SURVEY.md 8d "synthetic inputs"):

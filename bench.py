@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the AudioLDM2 sampling hot path (BASELINE.json metric: 10 s clips/sec @ 200 DDIM steps).
 
-    python bench.py --gpus N --steps K --warmup W            # native sm_100a engine (one rank per GPU)
+    python bench.py --gpus N --steps K --warmup W            # native sm_90a engine (one rank per GPU)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's own code on the host cores
 
 A "step" is one pass of the hot path over one batch: x_T -> 200 x (cond+uncond UNet, CFG, DDIM update)
@@ -13,7 +13,7 @@ checkpoints / tokenizers are unreachable; SURVEY.md 8d).  Conditioning encoders 
 the timed region (out of scope for this path).
 
 The native arm (N = 1) also times, in the same process and on the same GPU, the reference's own PyTorch-CUDA path
-(`torch_cuda_baseline`: unmodified reference modules from baseline/_ref when present, else the oracle port; two
+(`torch_cuda_baseline`: unmodified reference modules from oracle/_ref when present, else the oracle port; two
 apply_model calls per step as ddim.py:293-296) and reports `vs_torch_cuda` -- the north star's >= 4x target.
 """
 from __future__ import annotations
@@ -53,6 +53,8 @@ def parse():
     ap.add_argument("--no-torch-cuda-baseline", action="store_true")
     ap.add_argument("--ref-full", action="store_true", help="torch-CUDA baseline: run all DDIM steps for every precision mode")
     ap.add_argument("--dump-ops", default=None, help="write the per-op timing table of one UNet evaluation to this CSV")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the waveform batch of the last timed step to DIR/waveform.npy (float32; rank r > 0: waveform_rank<r>.npy)")
     return ap.parse_args()
 
 
@@ -73,7 +75,7 @@ def workload(a, cfg) -> str:
 
 
 # ------------------------------------------------------------------------------------------------
-# clocks: sample nvidia-smi DURING the timed region (B200_PROFILING.md)
+# clocks: sample nvidia-smi DURING the timed region
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -113,7 +115,7 @@ class ClockSampler:
 
 
 # ------------------------------------------------------------------------------------------------
-# CPU arm: the reference's own modules (baseline/_ref) or the oracle port on the host cores.  Clips are independent,
+# CPU arm: the reference's own modules (oracle/_ref) or the oracle port on the host cores.  Clips are independent,
 # so the host is filled with W worker processes x T intra-op threads, each sampling B = 1.
 # ------------------------------------------------------------------------------------------------
 def _cpu_worker(conn, model_name, t5_len, threads, seed, cpus):
@@ -168,7 +170,7 @@ class CpuPool:
 
     def calibrate(self, S: int):
         """How many of the spawned workers to run at once.  The logical-CPU count of a container says nothing about its CPU
-        quota (the GPU box reports 128 logical CPUs; 8 concurrent 16-thread workers each ran 10x slower than one alone), so
+        quota (on a host reporting 128 logical CPUs, 8 concurrent 16-thread workers each ran 10x slower than one alone), so
         the whole-host throughput of 1, 2, 4, ... concurrent workers is measured on one DDIM step and the best count kept."""
         trials, k = {}, 1
         while True:
@@ -325,17 +327,40 @@ def kernel_pass(eng, peaks: dict, dump=None):
                             f"{4.0 * o['B'] * o['heads'] * o['Nq'] * o['Nk'] * 32 / (ms * 1e-3) / 1e12:.1f}\n")
                 else:
                     f.write(f"{i},{o['kind']},{o.get('tag', 0)},{ms:.4f},{o.get('rows', 0)},{o.get('c0', 0)},0,0,0,0,0\n")
-    peak = peaks.get("bf16_tflops_sustained") or 1432.6
+    peak = peaks.get("bf16_tflops_sustained") or 989.4      # H100 SXM data sheet, dense FP16/BF16
     ach = fl / (tm * 1e-3) / 1e12 if tm > 0 else 0.0
     return dict(bound="tensor", achieved=ach, peak=peak, unit="TFLOP/s", frac=ach / peak, traffic=None,
-                kernel="gemm_tc3_kernel (persistent tcgen05 implicit GEMM)", gemm_flop_per_lane_eval=fl,
+                kernel="gemm_tc3_kernel (persistent wgmma implicit GEMM)", gemm_flop_per_lane_eval=fl,
                 peak_source=("MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "fallback"),
                 share_of_unet_step={k: round(v / total, 4) for k, v in per_kind.items()},
                 unet_eval_ms_eager=round(total, 3), lane_rows=pl.meta.get("Bt"))
 
 
+DUMP_BYTES = 64 << 20      # --dump-outputs: at most this much in all ranks' files together
+
+
+def dump_outputs(dirname: str, wave: torch.Tensor, rank: int, world: int):
+    """The last timed step's waveform batch as its caller receives it (the seeds make the inputs identical from run to run):
+    DIR/waveform.npy (rank r > 0: waveform_rank<r>.npy), float32.  When the ranks' waveforms together exceed DUMP_BYTES,
+    each rank writes a fixed, evenly spaced sample of its flattened waveform instead, with the flat indices in
+    waveform_index.npy (float64; every index is exact)."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    sfx = "" if rank == 0 else f"_rank{rank}"
+    x = wave.reshape(-1).numpy()
+    cap = DUMP_BYTES // (4 * world)
+    if x.size > cap:
+        cap //= 3                                    # sample (4 B) + its index (8 B) per element
+        idx = np.arange(cap, dtype=np.int64) * x.size // cap
+        np.save(os.path.join(dirname, f"waveform_index{sfx}.npy"), idx.astype(np.float64))
+        x = x[idx]
+    np.save(os.path.join(dirname, f"waveform{sfx}.npy"), x.reshape(wave.shape) if x.size == wave.numel() else x)
+
+
 def main():
     a = parse()
+    if a.steps < 1:
+        raise SystemExit("bench.py: --steps must be at least 1")
     if a.impl == "reference":
         return run_reference_arm(a)
     from audioldm2_b200 import arch, engine, frontend, model, parallel, synth
@@ -410,6 +435,8 @@ def main():
         wave_host.copy_(w, non_blocking=True)
     t_e2e = timed(e2e_step, a.steps)
     clk = clocks.stop() if rank == 0 else None
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, wave_host, rank, world)
 
     # phase breakdown + the waveform used for the parity figure against the reference's CUDA path (outside the timed regions)
     PSEED = 4242
@@ -448,13 +475,6 @@ def main():
     except Exception:
         pass
     roof = None if a.no_kernel_pass else kernel_pass(eng, peaks, a.dump_ops)
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        if roof is not None:
-            roof["traffic"] = tr.get("gemm_tc_kernel_dram_bytes_per_launch")
-            roof["traffic_source"] = tr.get("source", "profiles/traffic.json")
-    except Exception:
-        pass
     if roof is not None and breakdown.get("ms_per_ddim_step"):
         # `achieved` divides by per-op event times of an EAGER pass of one lane (every op carries a launch gap).  The same FLOPs
         # (all lanes) over the whole measured graph-replay step -- GEMMs, attention, norms and gaps included -- bound it from below.
@@ -486,7 +506,7 @@ def main():
                 dtype="f16x2 (split-fp16 tensor-core operands: weights hi + lo, activations hi + lo in the convolutions and one plane on the token side; fp32 accumulate, fp32 residual stream)", data="synthetic",
                 config=dict(workload=workload(a, cfg), lanes=lanes_used,
                             l2="no explicit flush: the UNet weights (1.39 GB for audioldm2-full) are re-streamed every DDIM step "
-                               "(working set >> 126 MB L2)",
+                               "(working set >> 50 MB L2)",
                             parallelism=f"dp{world} (contiguous shards of the global batch of {Bg}, weights broadcast once over NCCL, "
                                         "no per-step collective)"),
                 e2e=dict(value=e2e_value, unit=UNIT, h2d_bytes_per_step=h2d, d2h_bytes_per_step=wave_host.numel() * 4),
@@ -495,7 +515,9 @@ def main():
         line["torch_cuda_baseline"] = tcb
         if "high" in tcb:
             line["vs_torch_cuda"] = dict(ratio=value / tcb["high"]["value"], e2e_ratio=e2e_value / tcb["high"]["value"],
-                                         against="high (the reference as shipped: TF32 matmuls + TF32 convs)",
+                                         against=("high (the reference as shipped: TF32 matmuls + TF32 convs)" if tcb.get("kind") == "reference" else
+                                                  "high, run by oracle/functional.py (this project's restatement of the reference modules, "
+                                                  "used when no reference checkout was staged into oracle/_ref): TF32 matmuls + TF32 convs"),
                                          ratio_vs_default=value / tcb["default"]["value"], ratio_vs_fp32=value / tcb["fp32"]["value"])
     print(json.dumps(line))
 

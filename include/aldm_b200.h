@@ -1,11 +1,11 @@
 /*
- * aldm_b200.h -- C-ABI of the B200-native AudioLDM2 sampling hot path.
+ * aldm_b200.h -- C-ABI of the native AudioLDM2 sampling hot path (H100, sm_90a).
  *
  * Drop-in boundary (SURVEY.md 8b).  The reference (haoheliu/AudioLDM2) is pure Python/PyTorch;
  * its "FFI" for this path is the set of torch module calls listed below.  A Python host
  * (audioldm2_b200/engine.py, bound with ctypes -- see INTEGRATION.md) builds a flat table of
  * `aldm_op` records from the reference config dicts + state_dict and hands it to this library;
- * everything that touches the mel-latent tensor then runs as hand-written sm_100a kernels.
+ * everything that touches the mel-latent tensor then runs as hand-written sm_90a kernels.
  *
  *   reference call (file:line)                                   replaced by
  *   -----------------------------------------------------------  ---------------------------------
@@ -48,7 +48,7 @@
 extern "C" {
 #endif
 
-#define ALDM_ABI_VERSION 6
+#define ALDM_ABI_VERSION 7
 #define ALDM_MAX_TAPS 16
 
 enum {
@@ -63,7 +63,7 @@ enum {
 
 /* ---- GEMM / implicit-GEMM convolution ---------------------------------------------------- */
 
-enum { ALDM_GEMM_TC = 0, ALDM_GEMM_SIMT = 1, ALDM_GEMM_TC_V1 = 2 };   /* aldm_gemm_desc.impl: persistent tcgen05 | CUDA-core checker | one-tile-per-CTA tcgen05 */
+enum { ALDM_GEMM_TC = 0, ALDM_GEMM_SIMT = 1, ALDM_GEMM_TC_V1 = 2 };   /* aldm_gemm_desc.impl: persistent wgmma | CUDA-core checker | retired, selects the persistent kernel */
 /* OR-ed into aldm_gemm_desc.impl: w_packed is never written while the program runs (model weights), so the
  * kernel may start streaming it before its programmatic-dependency wait (overlapping the previous kernel's tail). */
 #define ALDM_GEMM_STATIC_B (1 << 16)
@@ -155,7 +155,7 @@ int aldm_pack_b(const float* src, int32_t lds, int32_t transpose, int32_t N, int
  * kv batch index bkv = b % kv_bmod (0: bkv = b).  mask: [Bkv, Nk] floats (1 = keep) or NULL; entries != 1
  * are filled with -FLT_MAX before the softmax exactly like attention.py:356-360.
  * Output: operand planes [B*Nq, ldo], head h at columns [h*32, +32).
- * impl: ALDM_GEMM_TC = tcgen05 flash kernel, ALDM_GEMM_SIMT = CUDA-core checker. */
+ * impl: ALDM_GEMM_TC = wgmma flash kernel, ALDM_GEMM_SIMT = CUDA-core checker. */
 typedef struct aldm_attn_desc {
   const void* q_hi; const void* q_lo; const void* k_hi; const void* k_lo; const void* vt_hi; const void* vt_lo;
   const float* mask;
@@ -258,7 +258,7 @@ typedef struct aldm_engine aldm_engine;
 
 /* One UNet lane: an independent copy of the step / conditioning programs planned for B / n_lanes latent rows, with
  * its own workspace (the weight arena is shared).  Lanes are replayed as PARALLEL branches of one CUDA graph: the
- * UNet's deep levels are chains of ~10 us kernels that each fill a fraction of the 148 SMs, so independent
+ * UNet's deep levels are chains of short kernels that each fill a fraction of the SMs, so independent
  * sub-batches overlap there while the large layers simply share the machine.  Samples are independent through the
  * whole path (SURVEY.md 8e), so results do not depend on the lane count (up to split-K / tile-shape choices). */
 typedef struct aldm_unet_lane {
@@ -319,9 +319,8 @@ size_t aldm_sizeof_gemm_desc(void);
 size_t aldm_sizeof_engine_desc(void);
 size_t aldm_offsetof_gemm(int32_t field);     /* 0:B 1:ntaps 2:dy 3:N 4:ldo 5:act 6:alpha 7:n_split (layout self-check) */
 const char* aldm_last_error(void);
-int aldm_device_check(int32_t device);
-int aldm_debug_timeline(long long* host_out, int32_t n);   /* profiling aid: per-stage clock64 stamps of CTA 0 (scripts/prof_ops.py --timeline) */        /* 0 if `device` is sm_100 and kernels can load */
-int aldm_debug_umma_rate(int32_t N, int32_t mode, int32_t reps, long long* host_out, int32_t n_out);   /* profiling aid: cycles for `reps` tcgen05.mma 128 x N x 16 on each of n_out SMs (scripts/umma_rate.py) */
+int aldm_device_check(int32_t device);   /* 0 if `device` is sm_90 and kernels can load */
+int aldm_debug_timeline(long long* host_out, int32_t n);   /* profiling aid: per-stage clock64 stamps of CTA 0 (scripts/prof_ops.py --timeline) */
 int aldm_debug_store_rate(int32_t n_cta, int32_t iters, int32_t mode, long long region_bytes, long long* host_out);   /* profiling aid: SM -> L2 store throughput, STG.128 (0) vs TMA bulk store (1) (scripts/store_rate.py) */
 
 #ifdef __cplusplus

@@ -3,9 +3,9 @@
 This is the oracle of SURVEY.md 8(c): a plain functional restatement of what the reference
 modules compute, driven by a ``state_dict`` with the reference key names.  It is pinned
 against the *unmodified imported reference modules* by ``tests/golden/make_golden.py``
-(run in the build container, where /root/reference exists); the committed fixtures under
+(run where a checkout of the reference is available); the committed fixtures under
 ``tests/golden/`` carry the reference outputs so the pin is re-checked on every test run
-(tests/test_oracle.py) and on the GPU box, where the reference is absent.
+(tests/test_oracle.py) without the reference.
 
 Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s cpu_baseline / --impl
 reference legs may import this module.  The product path (audioldm2_b200/*) never does.

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE -- CPU restatement of the STFT / mel front end (SURVEY.md 8a row A12).
 
 PARITY UNPINNED for the mel filterbank: the arithmetic lives in the third-party dependency
-``librosa==0.9.2`` (pinned in the reference's setup.py:48, not vendored in /root/reference,
+``librosa==0.9.2`` (pinned in the reference's setup.py:48, not vendored in the reference,
 not installed here).  ``mel_filterbank`` restates librosa 0.9.2's published algorithm
 (``librosa.filters.mel`` with its defaults ``htk=False, norm="slaney"``), which is what the
 reference call site ``librosa_mel_fn(sampling_rate, filter_length, n_mel_channels, mel_fmin,

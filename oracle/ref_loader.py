@@ -1,11 +1,10 @@
 """TEST INFRASTRUCTURE -- never imported by the product path.
 
-Imports the *unmodified* reference hot-path modules from ``/root/reference`` with the
-package ``__init__`` files bypassed (``audioldm2/__init__.py`` pulls in soundfile,
-progressbar, phonemizer ... which are not installed; SURVEY.md 8c).  Only usable in the
-build container: ``/root/reference`` does not exist on the GPU box, so this module is
-used exclusively by ``tests/golden/make_golden.py`` to generate the committed fixtures
-(and by an optional CPU test that is skipped when the reference is absent).
+Imports the *unmodified* reference hot-path modules from a checkout of the reference project
+(``$ALDM_REFERENCE_ROOT``, default ``oracle/_ref``, git-ignored) with the package ``__init__``
+files bypassed (``audioldm2/__init__.py`` pulls in soundfile, progressbar, phonemizer ... which
+are not installed; SURVEY.md 8c).  Used by ``tests/golden/make_golden.py`` to generate the
+committed fixtures; no test needs it.
 """
 from __future__ import annotations
 
@@ -14,7 +13,7 @@ import os
 import sys
 import types
 
-REF_ROOT = os.environ.get("ALDM_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("ALDM_REFERENCE_ROOT") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref")
 
 
 def available() -> bool:

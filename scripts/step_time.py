@@ -1,5 +1,5 @@
 """ms per DDIM step of the native engine for one configuration (env switches are read at plan / first-launch time, so
-every configuration runs in its own process; scripts/gpu_run.sh sweeps).  Prints one JSON line.
+every configuration runs in its own process).  Prints one JSON line.
 
     [ALDM_GN_FUSED=1] [ALDM_BN256=1] python scripts/step_time.py --lanes 2 [--batch 8] [--steps 40] [--model audioldm2-full]
 """

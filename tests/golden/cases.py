@@ -12,8 +12,46 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SAMPLER_SEED = 42          # pipeline.py:185 default seed
 
 
+class Sampled:
+    """A fixture tensor kept as an evenly spaced sample of its flattened elements (the full-size outputs would make the
+    fixture files too large to keep in the repository).  ``rel_l2`` (tests/conftest.py) compares the same elements of
+    the computed tensor; ``s[b]`` restricts the sample to one index of the leading dimension."""
+
+    def __init__(self, values: torch.Tensor, shape, idx: torch.Tensor = None):
+        self.shape = tuple(int(v) for v in shape)
+        numel = 1
+        for v in self.shape:
+            numel *= v
+        self.idx = sample_index(numel, values.numel()) if idx is None else idx
+        self.values = values
+
+    def take(self, x: torch.Tensor) -> torch.Tensor:
+        assert x.numel() == self.numel(), (tuple(x.shape), self.shape)
+        return x.reshape(-1)[self.idx.to(x.device)]
+
+    def numel(self) -> int:
+        n = 1
+        for v in self.shape:
+            n *= v
+        return n
+
+    def __getitem__(self, b: int) -> "Sampled":
+        row = self.numel() // self.shape[0]
+        sel = (self.idx // row) == b
+        return Sampled(self.values[sel], self.shape[1:], self.idx[sel] - b * row)
+
+
+def sample_index(numel: int, n: int) -> torch.Tensor:
+    """n evenly spaced flat indices out of numel (arithmetic only: the same on every torch version)."""
+    return torch.arange(n, dtype=torch.int64) * numel // n
+
+
 def load(name: str) -> dict:
-    return torch.load(os.path.join(HERE, name + ".pt"), map_location="cpu", weights_only=True)
+    d = torch.load(os.path.join(HERE, name + ".pt"), map_location="cpu", weights_only=True)
+    for k in [k for k in d if k.endswith(".shape")]:
+        key = k[:-len(".shape")]
+        d[key] = Sampled(d.pop(key + ".sample"), d.pop(k).tolist())
+    return d
 
 
 def latent(cfg: dict, B: int, seed: int = 3) -> torch.Tensor:

@@ -1,6 +1,6 @@
 """Generate the golden fixtures by running the UNMODIFIED reference modules.
 
-Run in the build container only (needs /root/reference):
+Run where the reference package is importable (oracle/ref_loader.py):
 
     python tests/golden/make_golden.py [--only NAME] [--skip-200]
 
@@ -30,9 +30,23 @@ from oracle import ref_loader                   # noqa: E402
 from tests.golden import cases                  # noqa: E402
 
 
+SAMPLE_BUDGET = 200_000      # float32 elements kept per fixture file: files stay under 1 MB
+
+
 def _save(name, d):
+    """Tensors of a fixture with more than SAMPLE_BUDGET elements in all are stored as evenly spaced samples
+    (``cases.Sampled``): ``<key>.sample`` + ``<key>.shape``."""
     path = os.path.join(HERE, name + ".pt")
-    torch.save({k: (v.contiguous() if torch.is_tensor(v) else v) for k, v in d.items()}, path)
+    big = {k: v for k, v in d.items() if torch.is_tensor(v) and v.is_floating_point() and v.numel() > 4096}
+    total = sum(v.numel() for v in big.values())
+    out = {k: (v.contiguous() if torch.is_tensor(v) else v) for k, v in d.items()}
+    if total > SAMPLE_BUDGET:
+        for k, v in big.items():
+            n = min(v.numel(), max(4096, SAMPLE_BUDGET * v.numel() // total))
+            del out[k]
+            out[k + ".sample"] = v.reshape(-1)[cases.sample_index(v.numel(), n)].clone()
+            out[k + ".shape"] = torch.tensor(list(v.shape), dtype=torch.int64)
+    torch.save(out, path)
     print(f"wrote {path} ({os.path.getsize(path) / 1e3:.0f} KB)")
 
 

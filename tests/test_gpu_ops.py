@@ -271,12 +271,12 @@ def test_gemm_vs_emulator(case, impl):
 @pytest.mark.parametrize("case", ["self", "self_long", "cross_mask", "cross_allmasked", "ragged", "bmod",
                                   "cross8_bmod", "cross32", "cross_tc_33"])
 def test_attention(case, impl):
-    """Q|K planes + transposed V planes -> attention kernel (tcgen05 / SIMT checker) vs the emulator."""
+    """Q|K planes + transposed V planes -> attention kernel (wgmma / SIMT checker) vs the emulator."""
     g = torch.Generator().manual_seed(5)
     P = Planner(impl=impl)
     B, heads = 3, 4
     Cc = heads * 32
-    # Nk <= 32 takes the CUDA-core short-key kernel (8 / 16 / 32 key instantiations), longer sets the tcgen05 kernel
+    # Nk <= 32 takes the CUDA-core short-key kernel (8 / 16 / 32 key instantiations), longer sets the wgmma kernel
     Nq, Nk = dict(self=(200, 200), self_long=(1024, 1024), cross_mask=(70, 9), cross_allmasked=(70, 9), ragged=(33, 130),
                   bmod=(64, 40), cross8_bmod=(300, 8), cross32=(130, 32), cross_tc_33=(130, 33))[case]
     Bkv = 1 if case.endswith("bmod") else B

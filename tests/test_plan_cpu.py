@@ -170,7 +170,7 @@ def test_half_width_tiles_rule():
     import math
     P = plan.Planner()
     mk = lambda N, K: torch.zeros(N, K)
-    assert P.wmat(mk(640, 640), None, 1, 640, m_rows=1024).bn == 64          # 40 tiles on 148 SMs, 10 k-blocks
+    assert P.wmat(mk(640, 640), None, 1, 640, m_rows=1024).bn == 64          # 40 tiles on 132 SMs, 10 k-blocks
     assert P.wmat(mk(640, 1280), None, 1, 1280, m_rows=1024).bn == 64
     assert P.wmat(mk(640, 5760), None, 9, 640, m_rows=1024).bn == 128        # long K: left to split-K
     assert P.wmat(mk(384, 384), None, 1, 384, m_rows=4096).bn == 128         # 96 tiles: halving would need a second wave
