@@ -24,13 +24,16 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-
 NVCC = shutil.which("nvcc") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
 
 MAX_TAPS = 16
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 # enums (keep in sync with the header; checked by tests/test_abi.py against the header text)
 GEMM_TC, GEMM_SIMT, GEMM_TC_V1 = 0, 1, 2
 GEMM_STATIC_B = 1 << 16
 ACT_NONE, ACT_GEGLU, ACT_TANH, ACT_SILU = 0, 1, 2, 3
 OUT_F32, OUT_PLANES, OUT_NCHW, OUT_QKV = 0, 1, 2, 3
+EPI_FAST, EPI_GEGLU, EPI_GENERIC, EPI_F32N, EPI_PLN = 0, 1, 2, 3, 4              # aldm_gemm_variant out[1]
+RED_NONE, RED_REDUCE4, RED_GENERIC = 0, 1, 2                                     # out[3]
+STORE_ROW, STORE_COMPACT, STORE_PAIR_PLN, STORE_PAIR_GEGLU, STORE_PAIR_QK = 0, 1, 2, 3, 4   # out[4]
 PREP_COPY, PREP_SILU, PREP_LRELU, PREP_GN, PREP_GN_SILU, PREP_LN = 0, 1, 2, 3, 4, 5
 OP_GEMM, OP_PREP, OP_ATTN, OP_SOFTMAX, OP_TEMB, OP_TRANSPOSE, OP_PACKB, OP_COPY = 1, 2, 3, 4, 5, 6, 7, 8
 
@@ -175,6 +178,7 @@ def lib() -> C.CDLL:
     vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
     sig = {
         "aldm_gemm": (i32, [C.POINTER(GemmDesc), vp]),
+        "aldm_gemm_variant": (i32, [C.POINTER(GemmDesc), C.POINTER(i32)]),
         "aldm_prep": (i32, [C.POINTER(PrepDesc), vp]),
         "aldm_pack_b": (i32, [vp, i32, i32, i32, i32, i32, vp, vp, vp]),
         "aldm_attention": (i32, [C.POINTER(AttnDesc), vp]),
@@ -226,7 +230,7 @@ def lib() -> C.CDLL:
     return L
 
 
-EXPORTED = ["aldm_gemm", "aldm_prep", "aldm_pack_b", "aldm_attention", "aldm_softmax_rows",
+EXPORTED = ["aldm_gemm", "aldm_gemm_variant", "aldm_prep", "aldm_pack_b", "aldm_attention", "aldm_softmax_rows",
             "aldm_timestep_embedding", "aldm_ddim_step", "aldm_masked_blend", "aldm_transpose_chw",
             "aldm_posterior_sample", "aldm_stft_mel", "aldm_program_create", "aldm_program_run",
             "aldm_program_run_range", "aldm_program_capture", "aldm_program_replay",
@@ -236,6 +240,13 @@ EXPORTED = ["aldm_gemm", "aldm_prep", "aldm_pack_b", "aldm_attention", "aldm_sof
             "aldm_sizeof_engine_desc", "aldm_abi_version", "aldm_sizeof_op",
             "aldm_sizeof_gemm_desc", "aldm_offsetof_gemm", "aldm_last_error", "aldm_device_check", "aldm_debug_timeline",
             "aldm_debug_store_rate"]
+
+
+def gemm_variant(d: GemmDesc) -> tuple:
+    """aldm_gemm_variant: (bn, epi, a_planes, reduction, store) of the kernel aldm_gemm runs for `d` (no GPU needed)."""
+    out = (C.c_int32 * 5)()
+    check(lib().aldm_gemm_variant(C.byref(d), out), "gemm_variant")
+    return tuple(out)
 
 
 def check(rc: int, what: str = ""):

@@ -374,7 +374,8 @@ __device__ long long g_timeline[4 * 256 * 2];
 // Tile order: split-K slice fastest, then n-tile, then m-tile, so CTAs running concurrently share the
 // same activation rows in L2.
 // ------------------------------------------------------------------------------------------
-enum { EPI_FAST = 0, EPI_GEGLU = 1, EPI_GENERIC = 2, EPI_F32N = 3, EPI_PLN = 4 };
+enum { EPI_FAST = ALDM_EPI_FAST, EPI_GEGLU = ALDM_EPI_GEGLU, EPI_GENERIC = ALDM_EPI_GENERIC, EPI_F32N = ALDM_EPI_F32N,
+       EPI_PLN = ALDM_EPI_PLN };
 
 // Division by a launch-time constant as multiply + shift (n < 2^31, d < 2^31): q = (n * M) >> (32 + l),
 // M = floor(2^(32+l) / d) + 1, l = ceil(log2 d).  The persistent roles run one warp per scheduler, so a
@@ -401,6 +402,7 @@ static FastDiv make_fastdiv(int d) {
 struct Tc3Divs {
   FastDiv ow, oh, cp, tn, bmod;
   int plain;      // 1x1 tap, unit stride, no upsample / batch-modulo: input row == output row (linear layers)
+  int store;      // ALDM_STORE_*: decided once on the host (gemm_select), so aldm_gemm_variant reports what runs
 };
 
 // AP = number of A planes (2: hi + lo, three MMAs per K step; 1: hi only, two MMAs and half the A bytes).
@@ -672,13 +674,10 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
         for (int ch = 0; ch < NRV; ++ch)
           if (has_res && half * 32 + 64 * ch < BN) co_load_res32(d, cr32, nt * BN + half * 32 + 64 * ch, d.N, lane, prv[ch]);
       }
-      // full-line pair mode (emit_pair_hi): single fp16 plane out, no residual, whole 64-column groups
-      const bool pair_pln = EPI == EPI_PLN && BN >= 64 && d.out_lo == nullptr && d.res == nullptr && d.splitk == 1 && d.N % 64 == 0 &&
-                            d.ldo % 8 == 0 && (reinterpret_cast<uintptr_t>(d.out_hi) & 15u) == 0;
-      const bool pair_geglu = EPI == EPI_GEGLU && BN == 128 && d.out_mode == ALDM_OUT_PLANES && d.out_lo == nullptr && d.splitk == 1 &&
-                              (d.N / 2) % 64 == 0 && d.ldo % 8 == 0 && (reinterpret_cast<uintptr_t>(d.out_hi) & 15u) == 0;
-      const bool pair_qk = EPI == EPI_FAST && BN >= 64 && d.out_mode == ALDM_OUT_QKV && d.out_lo == nullptr && d.res == nullptr &&
-                           d.splitk == 1 && d.n_split % 64 == 0 && d.ldo % 8 == 0 && (reinterpret_cast<uintptr_t>(d.out_hi) & 15u) == 0;
+      // full-line pair mode (emit_pair_hi): single fp16 plane out, no residual, whole 64-column groups (conditions: gemm_select)
+      const bool pair_pln = EPI == EPI_PLN && BN >= 64 && fd.store == ALDM_STORE_PAIR_PLN;
+      const bool pair_geglu = EPI == EPI_GEGLU && BN == 128 && fd.store == ALDM_STORE_PAIR_GEGLU;
+      const bool pair_qk = EPI == EPI_FAST && BN >= 64 && fd.store == ALDM_STORE_PAIR_QK;
       uint8_t* pair_tiles = reinterpret_cast<uint8_t*>(smem_raw + (bar_base + 256 - raw)) + (ew & 3) * (32 * 33 * 4);
       const int pair_bar = 1 + (ew & 3);
       float pln_b[NCH > 0 ? NCH : 1];      // bias of this warp's columns (lane = column), distributed by shuffles in pair mode
@@ -985,8 +984,51 @@ __global__ void gemm_simt_kernel(const __grid_constant__ aldm_gemm_desc d, int N
 // ------------------------------------------------------------------------------------------
 // host launch
 // ------------------------------------------------------------------------------------------
+// The kernel variant a descriptor runs: template parameters (BN, EPI, AP), split-K reduction kernel and store mode.  One
+// function decides it for the launch and for aldm_gemm_variant, so what the query reports is what runs.
+struct GemmVariant {
+  int bn, epi, ap, red, store;
+};
+
+static GemmVariant gemm_select(const aldm_gemm_desc& d) {
+  GemmVariant v{d.bn, EPI_GENERIC, d.a_lo ? 2 : 1, ALDM_RED_NONE, ALDM_STORE_ROW};
+  const int BN = d.bn;
+  // pick the specialised epilogue: the planner's dominant cases take the compact bodies
+  const bool geglu = d.act == ALDM_ACT_GEGLU;
+  const int n_out = geglu ? d.N / 2 : d.N;
+  const bool co = d.splitk == 1 && n_out % 4 == 0 && d.ldo % 4 == 0 && (!d.res || d.ld_res % 4 == 0) &&
+                  (d.out_mode == ALDM_OUT_F32 || d.out_mode == ALDM_OUT_PLANES || d.out_mode == ALDM_OUT_QKV);
+  const long long out_rows = (long long)d.B * d.OHF * d.OWF;
+  const int ld_max = d.ldo > d.ld_res ? d.ldo : d.ld_res;
+  static const bool compact_on = [] { const char* e = getenv("ALDM_EPI_COMPACT"); return !(e && e[0] == '0'); }();   // A/B switch
+  const bool plain = compact_on && co && d.act == ALDM_ACT_NONE && d.alpha == 1.0f && !d.accumulate && !d.rowvec &&
+                     out_rows * ld_max < (1ll << 31) &&
+                     (!d.bias || aligned16(d.bias)) && (!d.res || aligned16(d.res));
+  if (co && geglu && !d.res && d.out_mode != ALDM_OUT_QKV && BN >= 64) v.epi = EPI_GEGLU;
+  else if (plain && d.out_mode == ALDM_OUT_F32 && aligned16(d.out) && (!d.out_hi || d.ldo % 4 == 0)) v.epi = EPI_F32N;
+  else if (plain && d.out_mode == ALDM_OUT_PLANES) v.epi = EPI_PLN;
+  else if (co && d.act == ALDM_ACT_NONE) v.epi = EPI_FAST;
+  if (v.epi == EPI_F32N || v.epi == EPI_PLN) v.store = ALDM_STORE_COMPACT;
+  // full-line pair stores (emit_pair_hi): one fp16 plane out, no residual, whole 64-column groups, and every tile's columns
+  // inside the output (emit_pair_hi does not check them: N % BN == 0 for the planes form)
+  const bool pair_ok = d.out_lo == nullptr && d.splitk == 1 && d.ldo % 8 == 0 && aligned16(d.out_hi);
+  if (v.epi == EPI_PLN && BN >= 64 && pair_ok && d.res == nullptr && d.N % BN == 0) v.store = ALDM_STORE_PAIR_PLN;
+  if (v.epi == EPI_GEGLU && BN == 128 && pair_ok && d.out_mode == ALDM_OUT_PLANES && (d.N / 2) % 64 == 0) v.store = ALDM_STORE_PAIR_GEGLU;
+  if (v.epi == EPI_FAST && BN >= 64 && pair_ok && d.out_mode == ALDM_OUT_QKV && d.res == nullptr && d.n_split % 64 == 0)
+    v.store = ALDM_STORE_PAIR_QK;
+  if (d.splitk > 1) {
+    // coalesced reduction for the cases the planner actually splits; the row-owner kernel for everything else
+    const bool fast = d.act == ALDM_ACT_NONE && d.alpha == 1.0f && !d.accumulate && d.N % 4 == 0 && d.ldo % 4 == 0 &&
+                      (d.out_mode == ALDM_OUT_F32 || d.out_mode == ALDM_OUT_PLANES) && (!d.res || (d.ld_res % 4 == 0 && aligned16(d.res))) &&
+                      (!d.bias || aligned16(d.bias)) && (!d.rowvec || (d.ld_rowvec % 4 == 0 && aligned16(d.rowvec))) &&
+                      (d.out_mode != ALDM_OUT_F32 || aligned16(d.out));
+    v.red = fast ? ALDM_RED_REDUCE4 : ALDM_RED_GENERIC;
+  }
+  return v;
+}
+
 template <int BN, int EPI, int AP>
-static int launch_tc3_ap(const aldm_gemm_desc& d, int M, cudaStream_t st) {
+static int launch_tc3_ap(const aldm_gemm_desc& d, int M, const GemmVariant& v, cudaStream_t st) {
   using C = Tc3Cfg<BN, AP>;
   static bool configured = false;
   if (!configured) {
@@ -1001,18 +1043,15 @@ static int launch_tc3_ap(const aldm_gemm_desc& d, int M, cudaStream_t st) {
   fd.bmod = make_fastdiv(d.bmod > 0 ? d.bmod : 1);
   fd.plain = d.ntaps == 1 && d.dy[0] == 0 && d.dx[0] == 0 && d.sy == 1 && d.sx == 1 && d.up == 0 && d.bmod <= 0 &&
              d.OH == d.H && d.OW == d.W;
+  fd.store = v.store;
   ALDM_CHECK_CUDA(launch_pdl(gemm_tc3_kernel<BN, EPI, AP>, dim3(grid), dim3(416), C::SMEM_BYTES, st, d, tiles_m, tiles_n, fd));
   ALDM_CHECK_CUDA(cudaGetLastError());
   if (d.splitk > 1) {
     const int Mpad = tiles_m * C::BM, Npad = tiles_n * BN;
     const int chunks = (d.act == ALDM_ACT_GEGLU) ? (Npad / BN) * (BN / 64) : Npad / 32;
     const long long tot = (long long)M * chunks;
-    const bool fast = d.act == ALDM_ACT_NONE && d.alpha == 1.0f && !d.accumulate && d.N % 4 == 0 && d.ldo % 4 == 0 &&
-                      (d.out_mode == ALDM_OUT_F32 || d.out_mode == ALDM_OUT_PLANES) && (!d.res || (d.ld_res % 4 == 0 && aligned16(d.res))) &&
-                      (!d.bias || aligned16(d.bias)) && (!d.rowvec || (d.ld_rowvec % 4 == 0 && aligned16(d.rowvec))) &&
-                      (d.out_mode != ALDM_OUT_F32 || aligned16(d.out));
     // plain launches (full serialisation): early-scheduled reduction blocks only disturbed the GEMM's last epilogue
-    if (fast) {
+    if (v.red == ALDM_RED_REDUCE4) {
       const long long q = (long long)M * ((d.N + 3) / 4);
       splitk_reduce4_kernel<<<(unsigned)((q + 255) / 256), 256, 0, st>>>(d, Mpad, Npad);
     } else {
@@ -1024,37 +1063,27 @@ static int launch_tc3_ap(const aldm_gemm_desc& d, int M, cudaStream_t st) {
 }
 
 template <int BN, int EPI>
-static int launch_tc3_epi(const aldm_gemm_desc& d, int M, cudaStream_t st) {
-  return d.a_lo ? launch_tc3_ap<BN, EPI, 2>(d, M, st) : launch_tc3_ap<BN, EPI, 1>(d, M, st);
+static int launch_tc3_epi(const aldm_gemm_desc& d, int M, const GemmVariant& v, cudaStream_t st) {
+  return v.ap == 2 ? launch_tc3_ap<BN, EPI, 2>(d, M, v, st) : launch_tc3_ap<BN, EPI, 1>(d, M, v, st);
 }
 
 template <int BN>
-static int launch_tc2(const aldm_gemm_desc& d, int M, cudaStream_t st) {
-  // pick the specialised epilogue: the planner's dominant cases take the compact bodies
-  const bool geglu = d.act == ALDM_ACT_GEGLU;
-  const int n_out = geglu ? d.N / 2 : d.N;
-  const bool co = d.splitk == 1 && n_out % 4 == 0 && d.ldo % 4 == 0 && (!d.res || d.ld_res % 4 == 0) &&
-                  (d.out_mode == ALDM_OUT_F32 || d.out_mode == ALDM_OUT_PLANES || d.out_mode == ALDM_OUT_QKV);
-  if (co && geglu && !d.res && d.out_mode != ALDM_OUT_QKV && BN >= 64) return launch_tc3_epi<BN, EPI_GEGLU>(d, M, st);
-  const long long out_rows = (long long)d.B * d.OHF * d.OWF;
-  const int ld_max = d.ldo > d.ld_res ? d.ldo : d.ld_res;
-  static const bool compact_on = [] { const char* e = getenv("ALDM_EPI_COMPACT"); return !(e && e[0] == '0'); }();   // A/B switch
-  const bool plain = compact_on && co && d.act == ALDM_ACT_NONE && d.alpha == 1.0f && !d.accumulate && !d.rowvec &&
-                     out_rows * ld_max < (1ll << 31) &&
-                     (!d.bias || aligned16(d.bias)) && (!d.res || aligned16(d.res));
-  if (plain && d.out_mode == ALDM_OUT_F32 && aligned16(d.out) && (!d.out_hi || d.ldo % 4 == 0))
-    return launch_tc3_epi<BN, EPI_F32N>(d, M, st);
-  if (plain && d.out_mode == ALDM_OUT_PLANES) return launch_tc3_epi<BN, EPI_PLN>(d, M, st);
-  if (co && d.act == ALDM_ACT_NONE) return launch_tc3_epi<BN, EPI_FAST>(d, M, st);
-  return launch_tc3_epi<BN, EPI_GENERIC>(d, M, st);
+static int launch_tc2(const aldm_gemm_desc& d, int M, const GemmVariant& v, cudaStream_t st) {
+  switch (v.epi) {
+    case EPI_GEGLU: return launch_tc3_epi<BN, EPI_GEGLU>(d, M, v, st);
+    case EPI_F32N: return launch_tc3_epi<BN, EPI_F32N>(d, M, v, st);
+    case EPI_PLN: return launch_tc3_epi<BN, EPI_PLN>(d, M, v, st);
+    case EPI_FAST: return launch_tc3_epi<BN, EPI_FAST>(d, M, v, st);
+    default: return launch_tc3_epi<BN, EPI_GENERIC>(d, M, v, st);
+  }
 }
 
 int gemm_num_launches(const aldm_gemm_desc& d) { return ((d.impl & 0xff) != ALDM_GEMM_SIMT && d.splitk > 1) ? 2 : 1; }
 
-int gemm_launch(const aldm_gemm_desc& d, cudaStream_t st) {
+// descriptor checks shared by the launch and the variant query (no CUDA calls)
+static int gemm_check(const aldm_gemm_desc& d) {
   const long long Mll = (long long)d.B * d.OH * d.OW;
   ALDM_REQUIRE(Mll > 0 && Mll < (1ll << 31), ALDM_E_SHAPE, "gemm: bad M=%lld", Mll);
-  const int M = (int)Mll;
   ALDM_REQUIRE(d.bn == 32 || d.bn == 64 || d.bn == 128, ALDM_E_UNSUPPORTED, "gemm: bn=%d unsupported", d.bn);
   ALDM_REQUIRE(d.Cp % 8 == 0 && d.Cp > 0, ALDM_E_SHAPE, "gemm: Cp=%d must be a positive multiple of 8", d.Cp);
   ALDM_REQUIRE(d.ntaps >= 1 && d.ntaps <= ALDM_MAX_TAPS, ALDM_E_SHAPE, "gemm: ntaps=%d", d.ntaps);
@@ -1084,6 +1113,17 @@ int gemm_launch(const aldm_gemm_desc& d, cudaStream_t st) {
   }
   if ((d.impl & 0xff) == ALDM_GEMM_SIMT) {
     ALDM_REQUIRE(d.w_plain, ALDM_E_ARG, "gemm: SIMT path needs w_plain");
+  } else {
+    ALDM_REQUIRE(d.w_packed && aligned16(d.w_packed), ALDM_E_ARG, "gemm: w_packed null/unaligned");
+  }
+  return ALDM_OK;
+}
+
+int gemm_launch(const aldm_gemm_desc& d, cudaStream_t st) {
+  const int rc = gemm_check(d);
+  if (rc) return rc;
+  const int M = d.B * d.OH * d.OW;
+  if ((d.impl & 0xff) == ALDM_GEMM_SIMT) {
     const int Npad = cdiv(d.N, d.bn) * d.bn;
     const bool geglu = d.act == ALDM_ACT_GEGLU;
     const int nchunks = geglu ? (Npad / d.bn) * (d.bn / 64) : Npad / 32;
@@ -1092,12 +1132,12 @@ int gemm_launch(const aldm_gemm_desc& d, cudaStream_t st) {
     ALDM_CHECK_CUDA(cudaGetLastError());
     return ALDM_OK;
   }
-  ALDM_REQUIRE(d.w_packed && aligned16(d.w_packed), ALDM_E_ARG, "gemm: w_packed null/unaligned");
   // ALDM_GEMM_TC_V1 (the round-1 one-tile-per-CTA kernel) is retired: the value selects the persistent kernel
-  switch (d.bn) {
-    case 128: return launch_tc2<128>(d, M, st);
-    case 64: return launch_tc2<64>(d, M, st);
-    default: return launch_tc2<32>(d, M, st);
+  const GemmVariant v = gemm_select(d);
+  switch (v.bn) {
+    case 128: return launch_tc2<128>(d, M, v, st);
+    case 64: return launch_tc2<64>(d, M, v, st);
+    default: return launch_tc2<32>(d, M, v, st);
   }
 }
 
@@ -1110,6 +1150,16 @@ extern "C" int aldm_debug_timeline(long long* host_out, int32_t n) {
   void* sym = nullptr;        // cleared after every read so that stamps of different cases never mix
   ALDM_CHECK_CUDA(cudaGetSymbolAddress(&sym, g_timeline));
   ALDM_CHECK_CUDA(cudaMemset(sym, 0, sizeof(g_timeline)));
+  return ALDM_OK;
+}
+
+extern "C" int aldm_gemm_variant(const aldm_gemm_desc* d, int32_t out[5]) {
+  if (!d || !out) { aldm::set_error("aldm_gemm_variant: null argument"); return ALDM_E_ARG; }
+  const int rc = aldm::gemm_check(*d);
+  if (rc) return rc;
+  if ((d->impl & 0xff) == ALDM_GEMM_SIMT) { aldm::set_error("aldm_gemm_variant: the SIMT checker has no variants"); return ALDM_E_UNSUPPORTED; }
+  const aldm::GemmVariant v = aldm::gemm_select(*d);
+  out[0] = v.bn; out[1] = v.epi; out[2] = v.ap; out[3] = v.red; out[4] = v.store;
   return ALDM_OK;
 }
 

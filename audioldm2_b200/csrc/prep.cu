@@ -23,8 +23,25 @@ __device__ __forceinline__ float4 load_cat4(const aldm_prep_desc& d, long long r
   return *reinterpret_cast<const float4*>(d.src1 + row * d.c1 + (c - d.c0));
 }
 
+// GroupNorm statistics are accumulated relative to a pivot, the first element of the (batch, group) (row 0, channel g * cpg):
+// the per-thread fp32 sums of x and x^2 then hold values of the order of the group's spread rather than of its mean, so
+// var = E[(x-p)^2] - E[x-p]^2 does not cancel when |mean| >> std (offset activations).
+__device__ __forceinline__ float gn_pivot(const aldm_prep_desc& d, int b, int g, int cpg) {
+  const int c = g * cpg;
+  const long long row = (long long)b * d.HW;
+  return c < d.c0 ? __ldg(d.src0 + row * d.c0 + c) : __ldg(d.src1 + row * d.c1 + (c - d.c0));
+}
+// (sum, sumsq) of x - pivot over n elements -> mean, rstd
+__device__ __forceinline__ void gn_finish(double s, double s2, double n, float pivot, float eps, float& mean, float& rstd) {
+  const double ms = s / n;
+  double var = s2 / n - ms * ms;
+  if (var < 0.0) var = 0.0;
+  mean = (float)((double)pivot + ms);
+  rstd = (float)(1.0 / sqrt(var + (double)eps));
+}
+
 // ---------------------------------------------------------------------------------------------
-// GroupNorm statistics: grid (nblk, B); block 256.  partial[b][blk][g] = (sum, sumsq) as doubles.
+// GroupNorm statistics: grid (nblk, B); block 256.  partial[b][blk][g] = (sum, sumsq) of x - pivot as doubles.
 // ---------------------------------------------------------------------------------------------
 __global__ void gn_stats_kernel(const __grid_constant__ aldm_prep_desc d, int nblk) {
   pdl_wait();
@@ -37,7 +54,7 @@ __global__ void gn_stats_kernel(const __grid_constant__ aldm_prep_desc d, int nb
   const int r0 = blk * rows_per;
   const int r1 = min(d.HW, r0 + rows_per);
   const long long total = (long long)max(0, r1 - r0) * Q;
-  float acc = 0.f, acc2 = 0.f;
+  float acc = 0.f, acc2 = 0.f, pv = 0.f;
   int cur_g = -1;
   for (long long idx = threadIdx.x; idx < total; idx += blockDim.x) {
     const int pr = (int)(idx / Q), q = (int)(idx % Q);
@@ -50,9 +67,11 @@ __global__ void gn_stats_kernel(const __grid_constant__ aldm_prep_desc d, int nb
       if (g != cur_g) {
         if (cur_g >= 0) { atomicAdd(&s_sum[cur_g], (double)acc); atomicAdd(&s_sq[cur_g], (double)acc2); }
         cur_g = g; acc = 0.f; acc2 = 0.f;
+        pv = gn_pivot(d, b, g, cpg);
       }
-      acc += vv[e];
-      acc2 = fmaf(vv[e], vv[e], acc2);
+      const float x = vv[e] - pv;
+      acc += x;
+      acc2 = fmaf(x, x, acc2);
     }
   }
   if (cur_g >= 0) { atomicAdd(&s_sum[cur_g], (double)acc); atomicAdd(&s_sq[cur_g], (double)acc2); }
@@ -86,12 +105,7 @@ __global__ void gn_apply_kernel(const __grid_constant__ aldm_prep_desc d, int nb
       const double* p = d.scratch + (((long long)b * nblk_stats + k) * d.groups + threadIdx.x) * 2;
       s += p[0]; s2 += p[1];
     }
-    const double n = (double)d.HW * cpg;
-    const double mean = s / n;
-    double var = s2 / n - mean * mean;
-    if (var < 0.0) var = 0.0;
-    s_mean[threadIdx.x] = (float)mean;
-    s_rstd[threadIdx.x] = (float)(1.0 / sqrt(var + (double)d.eps));
+    gn_finish(s, s2, (double)d.HW * cpg, gn_pivot(d, b, threadIdx.x, cpg), d.eps, s_mean[threadIdx.x], s_rstd[threadIdx.x]);
   }
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
@@ -284,6 +298,7 @@ __global__ void __launch_bounds__(256) gn_stats_col_kernel(const __grid_constant
   pdl_wait();
   for (int q = q0; q < gg.Q; q += gg.QW) {
     float a = 0.f, a2 = 0.f;
+    const float pv = gn_pivot(d, b, (q * 4) / cpg, cpg);      // cpg % 4 == 0 on this path: one group per float4
     int r = r0 + slot;
     const long long rb = (long long)b * d.HW;
     for (; r + 3 * gg.RS < r1; r += 4 * gg.RS) {
@@ -292,12 +307,14 @@ __global__ void __launch_bounds__(256) gn_stats_col_kernel(const __grid_constant
       for (int u = 0; u < 4; ++u) v[u] = load_cat4(d, rb + r + u * gg.RS, q * 4);
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
+        v[u].x -= pv; v[u].y -= pv; v[u].z -= pv; v[u].w -= pv;
         a += (v[u].x + v[u].y) + (v[u].z + v[u].w);
         a2 = fmaf(v[u].x, v[u].x, fmaf(v[u].y, v[u].y, fmaf(v[u].z, v[u].z, fmaf(v[u].w, v[u].w, a2))));
       }
     }
     for (; r < r1; r += gg.RS) {
-      const float4 v = load_cat4(d, rb + r, q * 4);
+      float4 v = load_cat4(d, rb + r, q * 4);
+      v.x -= pv; v.y -= pv; v.z -= pv; v.w -= pv;
       a += (v.x + v.y) + (v.z + v.w);
       a2 = fmaf(v.x, v.x, fmaf(v.y, v.y, fmaf(v.z, v.z, fmaf(v.w, v.w, a2))));
     }
@@ -343,13 +360,8 @@ __global__ void __launch_bounds__(256) gn_stats_col_kernel(const __grid_constant
     if (threadIdx.x < 32) {
       s = 0.0; s2 = 0.0;
       for (int k = 0; k < nsl; ++k) { s += s_red[k][g][0]; s2 += s_red[k][g][1]; }
-      const double n = (double)d.HW * cpg;
-      const double mean = s / n;
-      double var = s2 / n - mean * mean;
-      if (var < 0.0) var = 0.0;
       float* st = gn_stats_ptr(d) + ((long long)b * 32 + g) * 2;
-      st[0] = (float)mean;
-      st[1] = (float)(1.0 / sqrt(var + (double)d.eps));
+      gn_finish(s, s2, (double)d.HW * cpg, gn_pivot(d, b, g, cpg), d.eps, st[0], st[1]);
     }
     if (threadIdx.x == 0) gn_ticket_ptr(d)[b] = 0u;      // self-resetting: the next GroupNorm starts from zero
   }
@@ -383,12 +395,7 @@ __global__ void __launch_bounds__(256) gn_apply_col_kernel(const __grid_constant
     if (threadIdx.x < 32) {
       s = 0.0; s2 = 0.0;
       for (int k = 0; k < nsl; ++k) { s += s_red[k][g][0]; s2 += s_red[k][g][1]; }
-      const double n = (double)d.HW * cpg;
-      const double mean = s / n;
-      double var = s2 / n - mean * mean;
-      if (var < 0.0) var = 0.0;
-      s_st[2 * g] = (float)mean;
-      s_st[2 * g + 1] = (float)(1.0 / sqrt(var + (double)d.eps));
+      gn_finish(s, s2, (double)d.HW * cpg, gn_pivot(d, b, g, cpg), d.eps, s_st[2 * g], s_st[2 * g + 1]);
     }
   } else if (threadIdx.x < 64) {
     s_st[threadIdx.x] = __ldcg(gn_stats_ptr(d) + (long long)b * 64 + threadIdx.x);
@@ -467,6 +474,7 @@ __global__ void __launch_bounds__(256) gn_fused_kernel(const __grid_constant__ a
   pdl_wait();
   float a = 0.f, a2 = 0.f;
   if (active) {
+    const float pv = gn_pivot(d, b, (c_base + q * 4) / cpg, cpg);      // cpg % 4 == 0 here: one group per float4
     int r = slot;
     constexpr int U = 8;        // independent 16-byte loads in flight per thread
     for (; r + (U - 1) * RS < d.HW; r += U * RS) {
@@ -476,15 +484,17 @@ __global__ void __launch_bounds__(256) gn_fused_kernel(const __grid_constant__ a
 #pragma unroll
       for (int u = 0; u < U; ++u) {
         gn_sx[(r + u * RS) * QW + q] = v[u];
-        a += (v[u].x + v[u].y) + (v[u].z + v[u].w);
-        a2 = fmaf(v[u].x, v[u].x, fmaf(v[u].y, v[u].y, fmaf(v[u].z, v[u].z, fmaf(v[u].w, v[u].w, a2))));
+        const float4 x = make_float4(v[u].x - pv, v[u].y - pv, v[u].z - pv, v[u].w - pv);
+        a += (x.x + x.y) + (x.z + x.w);
+        a2 = fmaf(x.x, x.x, fmaf(x.y, x.y, fmaf(x.z, x.z, fmaf(x.w, x.w, a2))));
       }
     }
     for (; r < d.HW; r += RS) {
       const float4 v = load_cat4(d, rb + r, c_base + q * 4);
       gn_sx[r * QW + q] = v;
-      a += (v.x + v.y) + (v.z + v.w);
-      a2 = fmaf(v.x, v.x, fmaf(v.y, v.y, fmaf(v.z, v.z, fmaf(v.w, v.w, a2))));
+      const float4 x = make_float4(v.x - pv, v.y - pv, v.z - pv, v.w - pv);
+      a += (x.x + x.y) + (x.z + x.w);
+      a2 = fmaf(x.x, x.x, fmaf(x.y, x.y, fmaf(x.z, x.z, fmaf(x.w, x.w, a2))));
     }
     s_a[slot * QW + q] = a;
     s_a2[slot * QW + q] = a2;
@@ -499,12 +509,7 @@ __global__ void __launch_bounds__(256) gn_fused_kernel(const __grid_constant__ a
         s += (double)s_a[sl * QW + g * qpg + k];
         s2 += (double)s_a2[sl * QW + g * qpg + k];
       }
-    const double n = (double)d.HW * cpg;
-    const double mean = s / n;
-    double var = s2 / n - mean * mean;
-    if (var < 0.0) var = 0.0;
-    s_mean[g] = (float)mean;
-    s_rstd[g] = (float)(1.0 / sqrt(var + (double)d.eps));
+    gn_finish(s, s2, (double)d.HW * cpg, gn_pivot(d, b, blockIdx.x * G + g, cpg), d.eps, s_mean[g], s_rstd[g]);
   }
   __syncthreads();
   if (!active) return;

@@ -344,12 +344,17 @@ class Planner:
         self.marks[name] = len(self.ops)
 
     # ---- ops -----------------------------------------------------------------------------
+    @staticmethod
+    def gn_scratch_bytes(B: int) -> int:
+        """Bytes of the GroupNorm scratch of a batch of B (layout: csrc/prep.cu): [B][64 blocks][32 groups][2] double
+        partials | [B][32][2] float (mean, rstd) | [B] uint tickets."""
+        return round_up(B * 64 * 32 * 2 * 8 + B * 32 * 2 * 4 + B * 4, ALIGN)
+
     def _gn_scratch(self, B: int) -> Ref:
-        # [B][64 blocks][32 groups][2] double partials | [B][32][2] float (mean, rstd) | [B] uint tickets.  The tickets must be
-        # ZERO when a GroupNorm starts (they reset themselves): the buffer therefore cannot come from the pool's free list --
-        # a hole there belongs to buffers that other ops rewrite on every run -- and is placed above the high-water mark by
-        # finish(), like the split-K scratch (the workspace is zero-initialised once by engine.DeviceProgram).
-        self._gn_scr[B] = round_up(B * 64 * 32 * 2 * 8 + B * 32 * 2 * 4 + B * 4, ALIGN)
+        # The tickets must be ZERO when a GroupNorm starts (they reset themselves): the buffer therefore cannot come from the
+        # pool's free list -- a hole there belongs to buffers that other ops rewrite on every run -- and is placed above the
+        # high-water mark by finish(), like the split-K scratch (the workspace is zero-initialised once by engine.DeviceProgram).
+        self._gn_scr[B] = self.gn_scratch_bytes(B)
         return "GNSCR%d" % B
 
     def prep(self, mode: int, src0: F32, src1: Optional[F32] = None, gamma: Optional[Ref] = None,

@@ -48,7 +48,7 @@
 extern "C" {
 #endif
 
-#define ALDM_ABI_VERSION 7
+#define ALDM_ABI_VERSION 8
 #define ALDM_MAX_TAPS 16
 
 enum {
@@ -115,6 +115,20 @@ typedef struct aldm_gemm_desc {
 } aldm_gemm_desc;
 
 int aldm_gemm(const aldm_gemm_desc* d, void* stream);
+
+/* Which tensor-core kernel variant aldm_gemm runs for `d` (host only, no GPU needed; the launch makes the same choice):
+ *   out[0] N tile (32 / 64 / 128)          out[1] epilogue body ALDM_EPI_*      out[2] A planes (1 / 2)
+ *   out[3] split-K reduction ALDM_RED_*    out[4] store mode ALDM_STORE_*
+ * Epilogue bodies: FAST (bias / row vector / residual, fp32 / planes / dual / QKV outputs), GEGLU, GENERIC (everything
+ * else, and every split-K GEMM), F32N / PLN (compact bodies: fp32 / plane output with bias and residual only).
+ * Reductions: REDUCE4 (coalesced, no activation / alpha / accumulate; fp32, planes or dual out), GENERIC (any epilogue).
+ * Store modes: ROW (per-warp rows), COMPACT (swizzled staging tile of the compact bodies), PAIR_* (two warps assemble
+ * full 128-byte fp16 lines: single-plane PLN output, GEGLU planes output, Q|K columns of a QKV output).
+ * Returns ALDM_E_UNSUPPORTED for the SIMT checker (impl = ALDM_GEMM_SIMT) and the aldm_gemm error for a bad descriptor. */
+enum { ALDM_EPI_FAST = 0, ALDM_EPI_GEGLU = 1, ALDM_EPI_GENERIC = 2, ALDM_EPI_F32N = 3, ALDM_EPI_PLN = 4 };
+enum { ALDM_RED_NONE = 0, ALDM_RED_REDUCE4 = 1, ALDM_RED_GENERIC = 2 };
+enum { ALDM_STORE_ROW = 0, ALDM_STORE_COMPACT = 1, ALDM_STORE_PAIR_PLN = 2, ALDM_STORE_PAIR_GEGLU = 3, ALDM_STORE_PAIR_QK = 4 };
+int aldm_gemm_variant(const aldm_gemm_desc* d, int32_t out[5]);
 
 /* ---- operand preparation (normalise / activate / split into bf16 hi+lo planes) ----------- */
 

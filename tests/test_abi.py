@@ -44,6 +44,11 @@ def test_enum_values_match_header():
     assert val("ALDM_GEMM_TC") == _lib.GEMM_TC and val("ALDM_GEMM_SIMT") == _lib.GEMM_SIMT and val("ALDM_GEMM_TC_V1") == _lib.GEMM_TC_V1
     assert [val("ALDM_ACT_NONE"), val("ALDM_ACT_GEGLU"), val("ALDM_ACT_TANH"), val("ALDM_ACT_SILU")] == [0, 1, 2, 3]
     assert [val("ALDM_OUT_F32"), val("ALDM_OUT_PLANES"), val("ALDM_OUT_NCHW")] == [0, 1, 2]
+    assert [val("ALDM_EPI_" + n) for n in ("FAST", "GEGLU", "GENERIC", "F32N", "PLN")] == \
+        [_lib.EPI_FAST, _lib.EPI_GEGLU, _lib.EPI_GENERIC, _lib.EPI_F32N, _lib.EPI_PLN]
+    assert [val("ALDM_RED_" + n) for n in ("NONE", "REDUCE4", "GENERIC")] == [_lib.RED_NONE, _lib.RED_REDUCE4, _lib.RED_GENERIC]
+    assert [val("ALDM_STORE_" + n) for n in ("ROW", "COMPACT", "PAIR_PLN", "PAIR_GEGLU", "PAIR_QK")] == \
+        [_lib.STORE_ROW, _lib.STORE_COMPACT, _lib.STORE_PAIR_PLN, _lib.STORE_PAIR_GEGLU, _lib.STORE_PAIR_QK]
     assert [val("ALDM_PREP_" + n) for n in ("COPY", "SILU", "LRELU", "GN", "GN_SILU", "LN")] == [0, 1, 2, 3, 4, 5]
     assert [val("ALDM_OP_" + n) for n in ("GEMM", "PREP", "ATTN", "SOFTMAX", "TEMB", "TRANSPOSE", "PACKB", "COPY")] == \
         [1, 2, 3, 4, 5, 6, 7, 8]
