@@ -2,7 +2,7 @@
 // written as the fp16 operand plane(s) the tensor-core GEMM consumes (hi, and lo unless out_lo == NULL).  All kernels are
 // HBM/L2-bound streaming kernels: float4 loads, 8/16-byte stores, warp-shuffle reductions.
 //
-//   GN  : gn_stats_kernel  (per-block fp32 partial sums -> double partials, no atomics, deterministic)
+//   GN  : gn_stats_kernel  (per-lane fp32 sums -> fixed-order double tree per block, no atomics, deterministic)
 //         gn_apply_kernel  (reduces the partials for its batch row, builds per-channel scale/shift
 //                           in shared memory, applies (+SiLU), splits, stores)
 //   LN  : ln_kernel        (one warp per token row, two-pass statistics in registers)
@@ -41,45 +41,41 @@ __device__ __forceinline__ void gn_finish(double s, double s2, double n, float p
 }
 
 // ---------------------------------------------------------------------------------------------
-// GroupNorm statistics: grid (nblk, B); block 256.  partial[b][blk][g] = (sum, sumsq) of x - pivot as doubles.
+// GroupNorm statistics (generic path, any channels per group): grid (nblk, B); block 256 = 8 warps; warp w owns groups
+// w, w + 8, ... of the block's rows.  Each lane accumulates its elements of the group in fp32, the lanes' sums are
+// combined as doubles by a fixed shuffle tree, so the result does not depend on scheduling.
+// partial[b][blk][g] = (sum, sumsq) of x - pivot as doubles.
 // ---------------------------------------------------------------------------------------------
 __global__ void gn_stats_kernel(const __grid_constant__ aldm_prep_desc d, int nblk) {
   pdl_wait();
-  __shared__ double s_sum[32], s_sq[32];
   const int b = blockIdx.y, blk = blockIdx.x;
-  const int C = d.c0 + d.c1, Q = C >> 2, cpg = C / d.groups;
-  if (threadIdx.x < 32) { s_sum[threadIdx.x] = 0.0; s_sq[threadIdx.x] = 0.0; }
-  __syncthreads();
+  const int C = d.c0 + d.c1, cpg = C / d.groups;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   const int rows_per = (d.HW + nblk - 1) / nblk;
   const int r0 = blk * rows_per;
   const int r1 = min(d.HW, r0 + rows_per);
-  const long long total = (long long)max(0, r1 - r0) * Q;
-  float acc = 0.f, acc2 = 0.f, pv = 0.f;
-  int cur_g = -1;
-  for (long long idx = threadIdx.x; idx < total; idx += blockDim.x) {
-    const int pr = (int)(idx / Q), q = (int)(idx % Q);
-    const long long row = (long long)b * d.HW + r0 + pr;
-    const float4 v = load_cat4(d, row, q * 4);
-    const float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int g = (q * 4 + e) / cpg;
-      if (g != cur_g) {
-        if (cur_g >= 0) { atomicAdd(&s_sum[cur_g], (double)acc); atomicAdd(&s_sq[cur_g], (double)acc2); }
-        cur_g = g; acc = 0.f; acc2 = 0.f;
-        pv = gn_pivot(d, b, g, cpg);
-      }
-      const float x = vv[e] - pv;
+  const int total = max(0, r1 - r0) * cpg;
+  for (int g = warp; g < d.groups; g += nwarps) {
+    const float pv = gn_pivot(d, b, g, cpg);
+    float acc = 0.f, acc2 = 0.f;
+    for (int idx = lane; idx < total; idx += 32) {
+      const long long row = (long long)b * d.HW + r0 + idx / cpg;
+      const int c = g * cpg + idx % cpg;
+      const float x = (c < d.c0 ? __ldg(d.src0 + row * d.c0 + c) : __ldg(d.src1 + row * d.c1 + (c - d.c0))) - pv;
       acc += x;
       acc2 = fmaf(x, x, acc2);
     }
-  }
-  if (cur_g >= 0) { atomicAdd(&s_sum[cur_g], (double)acc); atomicAdd(&s_sq[cur_g], (double)acc2); }
-  __syncthreads();
-  if (threadIdx.x < d.groups) {
-    double* p = d.scratch + (((long long)b * nblk + blk) * d.groups + threadIdx.x) * 2;
-    p[0] = s_sum[threadIdx.x];
-    p[1] = s_sq[threadIdx.x];
+    double s = acc, s2 = acc2;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      s += __shfl_xor_sync(0xffffffffu, s, o);
+      s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+    }
+    if (lane == 0) {
+      double* p = d.scratch + (((long long)b * nblk + blk) * d.groups + g) * 2;
+      p[0] = s;
+      p[1] = s2;
+    }
   }
 }
 

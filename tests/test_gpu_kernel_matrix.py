@@ -111,6 +111,12 @@ def _run_guarded(pl: plan.Plan, writes, wins, zero=(), scratch=()):
     before = ws.clone()
     prog.run("all")
     torch.cuda.synchronize()
+    _assert_unchanged(ws, before, wins, scratch)
+    return prog
+
+
+def _assert_unchanged(ws: torch.Tensor, before: torch.Tensor, wins, scratch=()):
+    """Every byte of `ws` outside the windows and the scratch regions equals `before`."""
     inside = torch.zeros_like(ws, dtype=torch.bool)
     for w in wins:
         w.mark(inside)
@@ -130,7 +136,6 @@ def _run_guarded(pl: plan.Plan, writes, wins, zero=(), scratch=()):
             where = f"{first - near.off - near.n_rows * near.ld * near.esz:+d} bytes past the end of the array at {near.off}"
         raise AssertionError(f"{stray.numel()} bytes changed outside the output windows; first at workspace byte {first}: "
                              f"{where}; scratch regions (first, last byte): {[(o, o + n - 1) for o, n in scratch]}")
-    return prog
 
 
 def _check(name: str, got: torch.Tensor, ref: torch.Tensor, planes: int, extra: Optional[torch.Tensor] = None):
