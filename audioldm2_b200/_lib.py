@@ -16,7 +16,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libaldm_b200.so")
-SOURCES = ["gemm.cu", "prep.cu", "attention.cu", "elementwise.cu", "stft.cu", "program.cu", "engine_abi.cu", "microbench.cu"]
+SOURCES = ["gemm.cu", "prep.cu", "attention.cu", "elementwise.cu", "stft.cu", "program.cu", "engine_abi.cu", "microbench.cu",
+           "cond/seqgen.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
@@ -24,18 +25,19 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-
 NVCC = shutil.which("nvcc") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
 
 MAX_TAPS = 16
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 # enums (keep in sync with the header; checked by tests/test_abi.py against the header text)
 GEMM_TC, GEMM_SIMT, GEMM_TC_V1 = 0, 1, 2
 GEMM_STATIC_B = 1 << 16
-ACT_NONE, ACT_GEGLU, ACT_TANH, ACT_SILU = 0, 1, 2, 3
+ACT_NONE, ACT_GEGLU, ACT_TANH, ACT_SILU, ACT_GELU_TANH = 0, 1, 2, 3, 4
 OUT_F32, OUT_PLANES, OUT_NCHW, OUT_QKV = 0, 1, 2, 3
 EPI_FAST, EPI_GEGLU, EPI_GENERIC, EPI_F32N, EPI_PLN = 0, 1, 2, 3, 4              # aldm_gemm_variant out[1]
 RED_NONE, RED_REDUCE4, RED_GENERIC = 0, 1, 2                                     # out[3]
 STORE_ROW, STORE_COMPACT, STORE_PAIR_PLN, STORE_PAIR_GEGLU, STORE_PAIR_QK = 0, 1, 2, 3, 4   # out[4]
 PREP_COPY, PREP_SILU, PREP_LRELU, PREP_GN, PREP_GN_SILU, PREP_LN = 0, 1, 2, 3, 4, 5
 OP_GEMM, OP_PREP, OP_ATTN, OP_SOFTMAX, OP_TEMB, OP_TRANSPOSE, OP_PACKB, OP_COPY = 1, 2, 3, 4, 5, 6, 7, 8
+OP_SEQ_ASSEMBLE, OP_KV_ATTN, OP_SEQ_FEEDBACK = 9, 10, 11
 
 
 class GemmDesc(C.Structure):
@@ -104,9 +106,27 @@ class _Copy(C.Structure):
     _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("bytes", C.c_int64)]
 
 
+class KvAttnDesc(C.Structure):
+    _fields_ = [("seq", C.c_void_p), ("mask", C.c_void_p), ("out_hi", C.c_void_p), ("out_lo", C.c_void_p),
+                ("B", C.c_int32), ("heads", C.c_int32), ("lmax", C.c_int32), ("ld_seq", C.c_int32), ("p0", C.c_int32),
+                ("nq", C.c_int32), ("ldo", C.c_int32), ("scale", C.c_float)]
+
+
+class SeqAssembleDesc(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("sos", C.c_void_p), ("eos", C.c_void_p), ("wpe", C.c_void_p), ("t5_mask", C.c_void_p),
+                ("mask", C.c_void_p), ("B", C.c_int32), ("L", C.c_int32), ("lmax", C.c_int32), ("C", C.c_int32)]
+
+
+class SeqFeedbackDesc(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p), ("wpe", C.c_void_p), ("out", C.c_void_p),
+                ("next", C.c_void_p), ("B", C.c_int32), ("nq", C.c_int32), ("C", C.c_int32), ("pos", C.c_int32),
+                ("k", C.c_int32), ("gen_len", C.c_int32), ("eps", C.c_float)]
+
+
 class _OpU(C.Union):
     _fields_ = [("gemm", GemmDesc), ("prep", PrepDesc), ("attn", AttnDesc), ("softmax", _Softmax),
-                ("temb", _Temb), ("transpose", _Transpose), ("packb", _PackB), ("copy", _Copy)]
+                ("temb", _Temb), ("transpose", _Transpose), ("packb", _PackB), ("copy", _Copy),
+                ("seq_assemble", SeqAssembleDesc), ("kv_attn", KvAttnDesc), ("seq_feedback", SeqFeedbackDesc)]
 
 
 class Op(C.Structure):
@@ -182,6 +202,9 @@ def lib() -> C.CDLL:
         "aldm_prep": (i32, [C.POINTER(PrepDesc), vp]),
         "aldm_pack_b": (i32, [vp, i32, i32, i32, i32, i32, vp, vp, vp]),
         "aldm_attention": (i32, [C.POINTER(AttnDesc), vp]),
+        "aldm_kv_attention": (i32, [C.POINTER(KvAttnDesc), vp]),
+        "aldm_seq_assemble": (i32, [C.POINTER(SeqAssembleDesc), vp]),
+        "aldm_seq_feedback": (i32, [C.POINTER(SeqFeedbackDesc), vp]),
         "aldm_softmax_rows": (i32, [vp, i32, i32, f32, vp, vp, vp]),
         "aldm_timestep_embedding": (i32, [vp, i32, i32, vp, vp, vp, vp]),
         "aldm_ddim_step": (i32, [vp, vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, vp]),
@@ -231,6 +254,7 @@ def lib() -> C.CDLL:
 
 
 EXPORTED = ["aldm_gemm", "aldm_gemm_variant", "aldm_prep", "aldm_pack_b", "aldm_attention", "aldm_softmax_rows",
+            "aldm_kv_attention", "aldm_seq_assemble", "aldm_seq_feedback",
             "aldm_timestep_embedding", "aldm_ddim_step", "aldm_masked_blend", "aldm_transpose_chw",
             "aldm_posterior_sample", "aldm_stft_mel", "aldm_program_create", "aldm_program_run",
             "aldm_program_run_range", "aldm_program_capture", "aldm_program_replay",

@@ -9,6 +9,7 @@ one description of the module tree.  Parameter names are the reference
 * UNet     : ``model.diffusion_model.``      (openaimodel.py:446-885)
 * VAE      : ``first_stage_model.``          (model.py:419-686, autoencoder.py:103-117)
 * vocoder  : ``first_stage_model.vocoder.``  (hifigan/models.py:112-174)
+* AudioMAE token generator: ``cond_stage_models.<i>.`` (audiomae_gen/sequence_input.py:11-60, HF GPT2Model)
 
 Nothing here touches torch; it is pure bookkeeping.
 """
@@ -348,3 +349,42 @@ def vocoder_out_len(cfg: dict, n_frames: int) -> int:
     for u, k in zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"]):
         L = (L - 1) * u - 2 * ((k - u) // 2) + k
     return L
+
+
+# --------------------------------------------------------------------------------------
+# AudioMAE token generator (SequenceGenAudioMAECond / Sequence2AudioMAE, audiomae_gen/sequence_input.py:11-60):
+# GPT-2 small (GPT2Config() defaults: 12 layers, 12 heads, width 768, 1024 positions, gelu_new, LayerNorm eps 1e-5),
+# input projections CLAP 512 -> 768 and Flan-T5 1024 -> 768, SOS / EOS embeddings nn.Embedding(32, 768).
+# --------------------------------------------------------------------------------------
+
+SEQGEN = dict(n_embd=768, n_head=12, n_positions=1024, vocab=50257, n_inner=3072, ln_eps=1e-5,
+              input_dims=(512, 1024), gen_len=8)          # sequence_input_embed_dim / sequence_gen_length (utils.py:362-368)
+
+
+def seqgen_param_shapes(n_layer: int = 12, with_wte: bool = True) -> Dict[str, Tuple[int, ...]]:
+    """name -> shape relative to ``cond_stage_models.<i>.``.  ``model.*`` are HF GPT-2 keys; its linear layers are
+    ``Conv1D`` with weights [in, out] (y = x W + b).  ``model.wte.weight`` is never read (inputs_embeds)."""
+    C, F = SEQGEN["n_embd"], SEQGEN["n_inner"]
+    P: Dict[str, Tuple[int, ...]] = {"model.wpe.weight": (SEQGEN["n_positions"], C)}
+    if with_wte:
+        P["model.wte.weight"] = (SEQGEN["vocab"], C)
+    for i in range(n_layer):
+        h = f"model.h.{i}"
+        for ln in ("ln_1", "ln_2"):
+            P[f"{h}.{ln}.weight"] = (C,); P[f"{h}.{ln}.bias"] = (C,)
+        for n, (k, o) in (("attn.c_attn", (C, 3 * C)), ("attn.c_proj", (C, C)), ("mlp.c_fc", (C, F)), ("mlp.c_proj", (F, C))):
+            P[f"{h}.{n}.weight"] = (k, o); P[f"{h}.{n}.bias"] = (o,)
+    P["model.ln_f.weight"] = (C,); P["model.ln_f.bias"] = (C,)
+    P["start_of_sequence_tokens.weight"] = (32, C)
+    P["end_of_sequence_tokens.weight"] = (32, C)
+    for j, d in enumerate(SEQGEN["input_dims"]):
+        P[f"input_sequence_embed_linear.{j}.weight"] = (C, d); P[f"input_sequence_embed_linear.{j}.bias"] = (C,)
+    return P
+
+
+def has_seqgen(cfg: dict) -> bool:
+    """Configs whose UNet reads ``crossattn_audiomae_generated`` (context 0 of width 768 next to a Flan-T5 context):
+    audioldm2-full and audioldm2-full-large.  audioldm_48k (FiLM only), the *_t5 models (T5 only) and the speech models
+    (phoneme-conditioned 512-token generation, not built here) have no such stage."""
+    dims = [c for c in (cfg["unet"].get("context_dim") or []) if c is not None]
+    return dims[:2] == [768, 1024] and "-speech-" not in cfg.get("name", "")

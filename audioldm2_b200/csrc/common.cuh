@@ -136,6 +136,12 @@ __device__ __forceinline__ float gelu_f(float x) {
   return 0.5f * x + 0.5f * fabsf(x) * erf_abs;     // 0.5 x (1 + sign(x) erf(|x|/sqrt2))
 }
 
+// GPT-2's gelu_new (activations.py NewGELUActivation): 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3))) with the accurate
+// tanhf, in the order of the module's expression.
+__device__ __forceinline__ float gelu_tanh_f(float x) {
+  return 0.5f * x * (1.0f + tanhf(0.7978845608028654f * (x + 0.044715f * (x * x * x))));
+}
+
 // v[i] *= gelu(g[i]) for NB values at once, written stage by stage so that NB independent dependency chains are in
 // flight: the GEGLU epilogue runs two warps per scheduler, and with the elements evaluated one or two at a time
 // (what the compiler produces from the scalar form under the 128-register cap) the dependency chain of each element

@@ -135,6 +135,9 @@ __device__ __forceinline__ void epi_activate(const aldm_gemm_desc& d, const RowI
   } else if (d.act == ALDM_ACT_SILU) {
 #pragma unroll
     for (int i = 0; i < 32; ++i) v[i] = silu_f(v[i]);
+  } else if (d.act == ALDM_ACT_GELU_TANH) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) v[i] = gelu_tanh_f(v[i]);
   }
 }
 

@@ -44,6 +44,9 @@ int gemm_num_launches(const aldm_gemm_desc& d);
 int prep_launch(const aldm_prep_desc& d, cudaStream_t st);
 int prep_num_launches(const aldm_prep_desc& d);
 int attention_launch(const aldm_attn_desc& d, cudaStream_t st);
+int kv_attention_launch(const aldm_kv_attn_desc& d, cudaStream_t st);
+int seq_assemble_launch(const aldm_seq_assemble_desc& d, cudaStream_t st);
+int seq_feedback_launch(const aldm_seq_feedback_desc& d, cudaStream_t st);
 
 }  // namespace aldm
 
@@ -72,6 +75,9 @@ static int run_op(const aldm_op& op, cudaStream_t st) {
     case ALDM_OP_PACKB:
       return aldm_pack_b(op.u.packb.src, op.u.packb.lds, op.u.packb.transpose, op.u.packb.N, op.u.packb.K, op.u.packb.bn,
                          op.u.packb.dst_packed, op.u.packb.dst_plain, st);
+    case ALDM_OP_SEQ_ASSEMBLE: return seq_assemble_launch(op.u.seq_assemble, st);
+    case ALDM_OP_KV_ATTN: return kv_attention_launch(op.u.kv_attn, st);
+    case ALDM_OP_SEQ_FEEDBACK: return seq_feedback_launch(op.u.seq_feedback, st);
     case ALDM_OP_COPY:
       ALDM_CHECK_CUDA(cudaMemcpyAsync(op.u.copy.dst, op.u.copy.src, (size_t)op.u.copy.bytes, cudaMemcpyDeviceToDevice, st));
       return ALDM_OK;

@@ -43,6 +43,27 @@ def split_state_dict(state_dict: Dict[str, torch.Tensor]):
     return un, vae, voc, sf
 
 
+def split_seqgen_state_dict(state_dict: Dict[str, torch.Tensor], index: int = 0) -> Dict[str, torch.Tensor]:
+    """The AudioMAE token generator's weights from a reference checkpoint: keys under ``cond_stage_models.<index>.``
+    (``index`` = position of ``crossattn_audiomae_generated`` in ``cond_stage_config``, 0 for audioldm2-full and -large),
+    restricted to arch.seqgen_param_shapes (the module's own CLAP / T5 / AudioMAE sub-models and the
+    ``attn.bias`` / ``attn.masked_bias`` buffers some transformers versions store are left out).  Raises if a key the
+    generator needs is missing.  ``split_state_dict`` is unchanged and does not return these."""
+    pre = f"cond_stage_models.{index}."
+    h = [k for k in state_dict if k.startswith(pre + "model.h.") and k.endswith(".ln_1.weight")]
+    n_layer = len(h)
+    want = arch.seqgen_param_shapes(n_layer, with_wte=False)
+    out = {}
+    for k, shp in want.items():
+        v = state_dict.get(pre + k)
+        if v is None:
+            raise KeyError(f"checkpoint has no {pre + k} (needed by the AudioMAE token generator)")
+        if tuple(v.shape) != tuple(shp):
+            raise ValueError(f"{pre + k}: shape {tuple(v.shape)}, expected {shp}")
+        out[k] = v
+    return out
+
+
 def reorder_cond_dict(cond_dict: dict, conditioning_key: Sequence[str]) -> dict:
     """LatentDiffusion.reorder_cond_dict (ddpm.py:1028-1032): the UNet consumes the conditions in the order of
     ``conditioning_key`` (the config's list), not in the dict's insertion order."""

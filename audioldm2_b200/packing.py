@@ -51,6 +51,12 @@ def conv_weight_matrix(w: torch.Tensor) -> Tuple[torch.Tensor, int, int]:
     return m.reshape(cout, taps * cp), taps, cp
 
 
+def conv1d_weight_matrix(w: torch.Tensor) -> Tuple[torch.Tensor, int, int]:
+    """HF ``Conv1D`` weight [in, out] (y = x W + b, the GPT-2 linear layers) -> ([out, Cp], 1 tap, Cp): the transpose of
+    a Linear weight, then the usual [N, K] matrix."""
+    return conv_weight_matrix(w.t().contiguous())
+
+
 def geglu_row_order(n_inner: int, bn: int) -> torch.Tensor:
     """Row permutation of GEGLU.proj ([2*n_inner, C]: values then gates, attention.py:42-44) so that every
     bn-row tile holds bn/2 value rows followed by their bn/2 gate rows."""

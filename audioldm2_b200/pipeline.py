@@ -4,11 +4,13 @@
 order and defaults (pipeline.py:142-267); extra keyword-only arguments configure what the reference obtains from the
 network.  What differs, by design of this tier:
 
-* the conditioning encoders (CLAP / Flan-T5 / AudioMAE-GPT2) are out of scope and need hub downloads that are
-  unreachable offline: the UNet-boundary conditioning comes from ``latent_diffusion.cond_provider`` (``.cond(batch)``
-  for the prompts, ``.uncond(n)`` for the unconditional branch); the default provider of a synthetic build is the
-  seeded one of SURVEY.md 8d.  A provider may return the reference's keyed cond-dict or the unpacked form
-  (model.unpack_cond_dict);
+* the conditioning encoders (CLAP / Flan-T5) are out of scope and need hub downloads that are unreachable offline:
+  conditioning comes from ``latent_diffusion.cond_provider`` (``.cond(batch)`` for the prompts, ``.uncond(n)`` for the
+  unconditional branch); the default provider of a synthetic build is the seeded one of SURVEY.md 8d.  A provider may
+  return the UNet-boundary conditioning (the reference's keyed cond-dict or the unpacked form, model.unpack_cond_dict),
+  or, for the sequence-generation models (audioldm2-full / -large), the encoder outputs ``film_clap_cond1`` [B, 1, 512]
+  and ``crossattn_flan_t5`` [h [B, L, 1024], mask [B, L]]: the AudioMAE tokens are then generated natively by GPT-2
+  (seqgen.NativeAudioMAEGenerator), on the B prompts before the n_gen tiling as in generate_batch (ddpm.py:1500-1523);
 * candidate re-ranking (ddpm.py:1554-1568) uses ``latent_diffusion.ranker(waveform [n,1,L], texts) -> similarity [n]``
   (the reference's ``clap.cos_similarity``); without one the first candidate of each prompt is returned and a
   warning says so;
@@ -41,6 +43,53 @@ class SyntheticConditioning:
         return synth.conditioning(self.cfg, n, seed=self.seed, t5_len=self.t5_len, device=self.device)[1]
 
 
+class SyntheticEncoderOutputs:
+    """Seeded encoder outputs for the sequence-generation models (opt-in; SyntheticConditioning stays the default): an
+    L2-normalised CLAP embedding [B, 1, 512] and Flan-T5 states N(0, 1) [B, L, 1024] with per-row lengths (row i holds
+    ``t5_lens[i % len]`` tokens, L = the longest, as padding=True pads to the longest prompt).  The unconditional branch
+    is SyntheticConditioning's single-prompt one repeated on every row (zero AudioMAE tokens, one T5("") row): like the
+    reference's, it does not depend on how many rows are asked for, so a rank of a sharded call sees the same rows as one
+    process."""
+
+    def __init__(self, cfg: dict, seed: int = 78, t5_lens=(32, 19, 7), t5_len: int = 32, device="cpu"):
+        if not arch.has_seqgen(cfg):
+            raise ValueError(f"{cfg.get('name')}: encoder outputs need the AudioMAE token generator, which this model has not")
+        self.cfg, self.seed, self.t5_lens, self.device = cfg, seed, tuple(t5_lens), device
+        self._uncond = SyntheticConditioning(cfg, t5_len=t5_len, device=device)
+
+    def cond(self, batch: dict) -> dict:
+        n = len(batch["text"])
+        clap, t5, mask = synth.encoder_outputs(n, [self.t5_lens[i % len(self.t5_lens)] for i in range(n)], seed=self.seed,
+                                               device=self.device)
+        return {"film_clap_cond1": clap, "crossattn_flan_t5": [t5, mask]}
+
+    def uncond(self, n: int) -> dict:
+        u = self._uncond.uncond(1)
+        return {k: ([t.expand(n, *t.shape[1:]).contiguous() for t in v] if isinstance(v, list) else
+                    (v.expand(n, *v.shape[1:]).contiguous() if torch.is_tensor(v) else v)) for k, v in u.items()}
+
+
+def is_encoder_level(cond: dict) -> bool:
+    """Encoder outputs rather than UNet-boundary conditioning: CLAP + Flan-T5 present, no AudioMAE tokens, not unpacked."""
+    return isinstance(cond, dict) and "film_clap_cond1" in cond and "crossattn_flan_t5" in cond and \
+        "crossattn_audiomae_generated" not in cond and "context_list" not in cond
+
+
+def route_conditioning(cfg: dict, cond: dict, generator: Callable[[], object]) -> dict:
+    """UNet-boundary conditioning is returned as it is (the generator is never built).  Encoder outputs go through
+    ``generator().generate`` -> {"crossattn_audiomae_generated": [tokens, ones], "crossattn_flan_t5": [h, mask]}, the
+    UNet's context order (SequenceGenAudioMAECond.forward, encoders/modules.py:281-300)."""
+    if not is_encoder_level(cond):
+        return cond
+    if not arch.has_seqgen(cfg):
+        raise ValueError(f"{cfg.get('name')} has no AudioMAE token generator: give UNet-boundary conditioning "
+                         "(context_list / crossattn_* entries), not CLAP + Flan-T5 encoder outputs")
+    h, m = cond["crossattn_flan_t5"]
+    tokens = generator().generate(cond["film_clap_cond1"], h, m)
+    return {"crossattn_audiomae_generated": [tokens, torch.ones(tokens.shape[:2], device=tokens.device)],
+            "crossattn_flan_t5": [h, m]}
+
+
 def _tile(c, n_gen: int):
     """The n_gen tiling of generate_batch (ddpm.py:1516-1525): torch.cat([t] * n_gen) on every tensor, so the candidates
     of prompt i sit at rows i + k * batchsize."""
@@ -70,7 +119,7 @@ class NativeAudioLDM2:
     ``generate_batch_masked``, ``latent_t_size``) over per-shape native engines."""
 
     def __init__(self, cfg: dict, unet_sd, vae_sd, vocoder_sd, device, scale_factor: float = 1.0, ctx_max_len=None,
-                 cond_provider=None, ranker: Optional[Callable] = None, **engine_kw):
+                 cond_provider=None, ranker: Optional[Callable] = None, seqgen_sd=None, **engine_kw):
         self.cfg, self.device = cfg, torch.device(device)
         self._sd = (unet_sd, vae_sd, vocoder_sd)
         self.scale_factor = scale_factor
@@ -81,6 +130,23 @@ class NativeAudioLDM2:
         self.cond_stage_key = "text"
         self._engines: Dict[Tuple[int, int, bool], model.NativeLatentDiffusion] = {}
         self._pinned: Dict[Tuple[int, ...], torch.Tensor] = {}
+        self._seqgen_sd = seqgen_sd
+        self._seqgen = None
+
+    # ---- AudioMAE token generator (built on first use: UNet-boundary providers never pay for it) ----------------------
+    def seqgen(self):
+        if self._seqgen is None:
+            if self._seqgen_sd is None:
+                raise ValueError("encoder-level conditioning needs the AudioMAE generator's weights (cond_stage_models.<i>.*), "
+                                 "which this model was built without")
+            from .seqgen import NativeAudioMAEGenerator
+            self._seqgen = NativeAudioMAEGenerator(self._seqgen_sd, self.device)
+        return self._seqgen
+
+    def conditioning(self, batch) -> dict:
+        """The provider's conditioning of the call's B prompts, with the AudioMAE tokens generated when it holds
+        encoder outputs."""
+        return route_conditioning(self.cfg, self.cond_provider.cond(batch), self.seqgen)
 
     # ---- engines -------------------------------------------------------------------------------------
     def engine(self, Bl: int, latent_t: Optional[int] = None, with_encoder: bool = False) -> model.NativeLatentDiffusion:
@@ -144,7 +210,7 @@ class NativeAudioLDM2:
         B = len(batch["text"])
         local = {k: (v[lo:hi] if (torch.is_tensor(v) or isinstance(v, list)) and len(v) == B else v) for k, v in batch.items()}
         rows = [i + k * B for k in range(n_gen) for i in range(lo, hi)]
-        cond_l = parallel.shard_rows(self.cond_provider.cond(batch), lo, hi)       # conditioning of the whole call, this rank's rows
+        cond_l = parallel.shard_rows(self.conditioning(batch), lo, hi)             # conditioning of the whole call, this rank's rows
         out = self._generate_local(local, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, (B, rows), cond_l)
         full = parallel.all_gather_rows(torch.from_numpy(out).to(self.device), B)
         return self._egress(full)
@@ -177,7 +243,7 @@ class NativeAudioLDM2:
             mask[:, int(T * tmask[0]):int(T * tmask[1]), :] = 0
             mask[:, :, int(F_ * fmask[0]):int(F_ * fmask[1])] = 0
             mask = mask[:, None].contiguous()
-        cond = _tile(cond_rows if cond_rows is not None else self.cond_provider.cond(batch), n_gen)
+        cond = _tile(cond_rows if cond_rows is not None else self.conditioning(batch), n_gen)
         if guidance != 1.0 and uncond is None:
             uncond = self.cond_provider.uncond(Bl)                                        # ddpm.py:1529-1536
         texts = list(batch["text"]) * n_gen
@@ -195,9 +261,11 @@ class NativeAudioLDM2:
 
 
 def build_model(ckpt_path=None, config=None, device=None, model_name="audioldm2-full", *, synthetic: Optional[bool] = None,
-                cond_provider=None, ranker: Optional[Callable] = None, t5_len: int = 32, ctx_max_len=None, **engine_kw):
+                cond_provider=None, ranker: Optional[Callable] = None, t5_len: int = 32, ctx_max_len=None, seqgen_index: int = 0,
+                **engine_kw):
     """pipeline.py:142-179.  ``ckpt_path`` is a reference ``<model_name>.pth`` (``["state_dict"]``, key layout of SURVEY.md
-    8b); without it (no network here, utils.py:209-219) the seeded synthetic checkpoint is used.  Engines are planned lazily
+    8b); without it (no network here, utils.py:209-219) the seeded synthetic checkpoint is used.  For audioldm2-full / -large
+    the AudioMAE generator's weights are taken too (``cond_stage_models.<seqgen_index>.``), for encoder-level providers.  Engines are planned lazily
     for the latent batch of each call (``batchsize * n_candidate_gen_per_text``)."""
     if device is None or device == "auto":
         device = torch.device("cuda:0")          # the native path has no CPU / MPS fallback
@@ -210,13 +278,15 @@ def build_model(ckpt_path=None, config=None, device=None, model_name="audioldm2-
             raise RuntimeError("no checkpoint given and hub download is unavailable offline (utils.py:209-219)")
         un, vae, voc, sf = synth.unet_state_dict(cfg["unet"]), synth.vae_state_dict(cfg["vae"]), \
             synth.vocoder_state_dict(cfg["vocoder"]), 1.0
+        seq = synth.seqgen_state_dict() if arch.has_seqgen(cfg) else None
         if ctx_max_len is None:
             n_cross = len([c for c in cfg["unet"]["context_dim"] if c is not None])
             ctx_max_len = (8, t5_len) if n_cross > 1 else (t5_len,)
     else:
         sd = torch.load(ckpt_path, map_location="cpu")["state_dict"]                      # pipeline.py:172
         un, vae, voc, sf = model.split_state_dict(sd)
-    ld = NativeAudioLDM2(cfg, un, vae, voc, device, scale_factor=sf, ctx_max_len=ctx_max_len,
+        seq = model.split_seqgen_state_dict(sd, seqgen_index) if arch.has_seqgen(cfg) else None
+    ld = NativeAudioLDM2(cfg, un, vae, voc, device, scale_factor=sf, ctx_max_len=ctx_max_len, seqgen_sd=seq,
                          cond_provider=cond_provider or SyntheticConditioning(cfg, t5_len=t5_len, device=device), ranker=ranker,
                          **engine_kw)
     ld.model_name = model_name

@@ -216,6 +216,29 @@ class Plan:
                 b = op.u.packb
                 b.src, b.dst_packed, b.dst_plain = P(o["src"]), P(o["dst_packed"]), P(o.get("dst_plain"))
                 b.lds, b.transpose, b.N, b.K, b.bn = int(o["lds"]), int(o["transpose"]), int(o["N"]), int(o["K"]), int(o["bn"])
+            elif k == "seq_assemble":
+                op.kind = _lib.OP_SEQ_ASSEMBLE
+                a = op.u.seq_assemble
+                for name in ("x", "sos", "eos", "wpe", "t5_mask", "mask"):
+                    setattr(a, name, P(o[name]))
+                for name in ("B", "L", "lmax", "C"):
+                    setattr(a, name, int(o[name]))
+            elif k == "kv_attn":
+                op.kind = _lib.OP_KV_ATTN
+                a = op.u.kv_attn
+                for name in ("seq", "mask", "out_hi", "out_lo"):
+                    setattr(a, name, P(o.get(name)))
+                for name in ("B", "heads", "lmax", "ld_seq", "p0", "nq", "ldo"):
+                    setattr(a, name, int(o[name]))
+                a.scale = float(o["scale"])
+            elif k == "seq_feedback":
+                op.kind = _lib.OP_SEQ_FEEDBACK
+                a = op.u.seq_feedback
+                for name in ("x", "gamma", "beta", "wpe", "out", "next"):
+                    setattr(a, name, P(o.get(name)))
+                for name in ("B", "nq", "C", "pos", "k", "gen_len"):
+                    setattr(a, name, int(o[name]))
+                a.eps = float(o["eps"])
             elif k == "copy":
                 op.kind = _lib.OP_COPY
                 c = op.u.copy
@@ -911,3 +934,141 @@ def build_vocoder(sd, cfg: dict, frames: int, batch: int, **pk) -> Plan:
     P.mark("end")
     io = dict(mel=("f32", mel_in.ref, (B, frames, nm)), wave=("f32", wave.ref, (B, 1, L)))
     return P.finish(io, meta=dict(B=B, L=L))
+
+
+# ==============================================================================================
+# AudioMAE token generator: GPT-2 with a KV cache (audiomae_gen/sequence_input.py:110-201,294-325)
+# ==============================================================================================
+SEQGEN_BN = 32       # N tile of every generator GEMM: the decode passes have M = B <= 8 rows, so the tile count (and with it
+                     # the number of SMs streaming the weights) is N / bn; the same packed weights serve prefill and decode
+
+
+@dataclass
+class SeqgenWeights:
+    """The generator's packed weight arena, planned once and shared by the plans of every (batch, T5 length)."""
+    arena: torch.Tensor
+    n_layer: int
+    refs: Dict[str, object]
+
+
+def pack_seqgen_weights(sd: Dict[str, torch.Tensor], **pk) -> SeqgenWeights:
+    """Weights of split_seqgen_state_dict / synth.seqgen_state_dict -> tile images.  Two planes everywhere (22-bit
+    weights; the activations are two-plane operands as well, DESIGN.md section 1).  ``model.wte`` is not uploaded."""
+    P = Planner(**pk)
+    n_layer = len([k for k in sd if k.startswith("model.h.") and k.endswith(".ln_1.weight")])
+    if n_layer == 0:
+        raise KeyError("state dict holds no GPT-2 layers (model.h.<i>.*)")
+    C = arch.SEQGEN["n_embd"]
+
+    def lin(w: torch.Tensor, b: torch.Tensor) -> WMat:          # nn.Linear [out, in]
+        wm, taps, cp = packing.conv_weight_matrix(w.float())
+        return P.wmat(wm, b, taps, cp, bn=SEQGEN_BN)
+
+    def c1d(n: str) -> WMat:                                     # HF Conv1D [in, out]
+        wm, taps, cp = packing.conv1d_weight_matrix(sd[n + ".weight"].float())
+        return P.wmat(wm, sd[n + ".bias"], taps, cp, bn=SEQGEN_BN)
+
+    r: Dict[str, object] = {
+        "wpe": P.vec(sd["model.wpe.weight"]),
+        "sos": P.vec(sd["start_of_sequence_tokens.weight"][:2]),
+        "eos": P.vec(sd["end_of_sequence_tokens.weight"][:2]),
+        "proj0": lin(sd["input_sequence_embed_linear.0.weight"], sd["input_sequence_embed_linear.0.bias"]),
+        "proj1": lin(sd["input_sequence_embed_linear.1.weight"], sd["input_sequence_embed_linear.1.bias"]),
+        "ln_f": (P.vec(sd["model.ln_f.weight"]), P.vec(sd["model.ln_f.bias"])),
+    }
+    for i in range(n_layer):
+        h = f"model.h.{i}"
+        r[f"{i}.ln_1"] = (P.vec(sd[h + ".ln_1.weight"]), P.vec(sd[h + ".ln_1.bias"]))
+        r[f"{i}.ln_2"] = (P.vec(sd[h + ".ln_2.weight"]), P.vec(sd[h + ".ln_2.bias"]))
+        for n in ("attn.c_attn", "attn.c_proj", "mlp.c_fc", "mlp.c_proj"):
+            r[f"{i}.{n}"] = c1d(f"{h}.{n}")
+    assert r["wpe"].off >= 0 and C == sd["model.wpe.weight"].shape[1]
+    return SeqgenWeights(P.arena.build(), n_layer, r)
+
+
+def build_seqgen(sd: Optional[Dict[str, torch.Tensor]], batch: int, t5_len: int, gen_len: int = 8,
+                 weights: Optional[SeqgenWeights] = None, **pk) -> Plan:
+    """Sequence2AudioMAE.generate for one (batch, T5 length L): the prefill pass over P = L + 5 positions, then
+    gen_len - 1 decode passes of one position each, all reading and extending per-layer KV caches.
+
+    io: clap [B, 1, 512], t5 [B, L, 1024], t5_mask [B, L] in; tokens [B, gen_len, 768] out.  Marks: "begin",
+    "prefill_end", "decode{k}_end" (k = 1 .. gen_len - 1), "end".  The plan references the arena of ``weights``
+    (packed from ``sd`` when None): plans of different shapes share one uploaded copy."""
+    W = weights if weights is not None else pack_seqgen_weights(sd, **pk)
+    P = Planner(**pk)
+    B, L = int(batch), int(t5_len)
+    C, H = arch.SEQGEN["n_embd"], arch.SEQGEN["n_head"]
+    Pn = L + 5
+    lmax = Pn + gen_len
+    if B < 1 or L < 1 or gen_len < 1:
+        raise ValueError(f"seqgen: batch {B}, T5 length {L}, gen_len {gen_len}")
+    if Pn > arch.SEQGEN["n_positions"] - gen_len:
+        raise ValueError(f"seqgen: {Pn} input positions + {gen_len} generated exceed GPT-2's "
+                         f"{arch.SEQGEN['n_positions']} positions (the reference would truncate; T5 inputs are <= 128 tokens)")
+    r = W.refs
+    eps = arch.SEQGEN["ln_eps"]
+    d0, d1 = arch.SEQGEN["input_dims"]
+    clap_in = F32(P.raw(B * d0 * 4), B, d0)
+    t5_in = F32(P.raw(B * L * d1 * 4), B * L, d1)
+    t5_mask = P.raw(B * L * 4)
+    tokens = P.raw(B * gen_len * C * 4)
+    mask = P.raw(B * lmax * 4)
+    seqs = [P.raw(B * lmax * 3 * C * 4) for _ in range(W.n_layer)]        # per-layer KV cache (q | k | v per position)
+    x_dec = F32(P.raw(B * C * 4), B, C)                                    # decode input: fed-back token + wpe
+    io = dict(clap=("f32", clap_in.ref, (B, 1, d0)), t5=("f32", t5_in.ref, (B, L, d1)), t5_mask=("f32", t5_mask, (B, L)),
+              tokens=("f32", tokens, (B, gen_len, C)))
+
+    P.mark("begin")
+    P.tag = 0
+    x = P.f32(B * Pn, C)
+    # the input projections write straight into their rows of the residual stream (rows 1 and [4, 4 + L) of each batch row)
+    cp = P.prep(_lib.PREP_COPY, clap_in)
+    P.gemm(cp, r["proj0"], B=B, H=1, out_ref=x.ref, ldo=C, OHF=Pn, ooy=1)
+    tp = P.prep(_lib.PREP_COPY, t5_in)
+    P.gemm(tp, r["proj1"], B=B, H=L, out_ref=x.ref, ldo=C, OHF=Pn, ooy=4)
+    P.free(cp, tp)
+    P.ops.append(dict(kind="seq_assemble", tag=0, x=x.ref, sos=r["sos"], eos=r["eos"], wpe=r["wpe"], t5_mask=t5_mask, mask=mask,
+                      B=B, L=L, lmax=lmax, C=C))
+
+    def gpt2_pass(xin: F32, p0: int, nq: int, k: int, last: bool):
+        """GPT2Model.forward over positions [p0, p0 + nq) of every batch row (HF GPT2Block: x += attn(ln_1(x));
+        x += mlp(ln_2(x))), then ln_f of the last position -> token k (+ wpe as the next pass's input)."""
+        R = B * nq
+        cur = xin
+        for i in range(W.n_layer):
+            P.tag = 1 + i
+            a = P.prep(_lib.PREP_LN, cur, None, *r[f"{i}.ln_1"], eps=eps)
+            P.gemm(a, r[f"{i}.attn.c_attn"], B=B, H=nq, out_ref=seqs[i], ldo=3 * C, OHF=lmax, ooy=p0)
+            P.free(a)
+            o = P.planes(R, C)
+            P.ops.append(dict(kind="kv_attn", tag=P.tag, seq=seqs[i], mask=mask, out_hi=o.hi, out_lo=o.lo, B=B, heads=H, lmax=lmax,
+                              ld_seq=3 * C, p0=p0, nq=nq, ldo=o.Cp, scale=1.0 / 8.0))
+            x2 = P.f32(R, C)
+            P.gemm(o, r[f"{i}.attn.c_proj"], B=1, H=R, out=x2, res=cur)
+            P.free(o)
+            if cur is not xin or xin is x:
+                P.free(cur)
+            a = P.prep(_lib.PREP_LN, x2, None, *r[f"{i}.ln_2"], eps=eps)
+            hmid = P.planes(R, arch.SEQGEN["n_inner"])
+            P.gemm(a, r[f"{i}.mlp.c_fc"], B=1, H=R, out_planes=hmid, act=_lib.ACT_GELU_TANH)
+            P.free(a)
+            x3 = P.f32(R, C)
+            P.gemm(hmid, r[f"{i}.mlp.c_proj"], B=1, H=R, out=x3, res=x2)
+            P.free(hmid, x2)
+            cur = x3
+        P.tag = 1 + W.n_layer
+        P.ops.append(dict(kind="seq_feedback", tag=P.tag, x=cur.ref, gamma=r["ln_f"][0], beta=r["ln_f"][1], wpe=r["wpe"],
+                          out=tokens, next=None if last else x_dec.ref, B=B, nq=nq, C=C, pos=p0 + nq - 1, k=k, gen_len=gen_len,
+                          eps=eps))
+        P.free(cur)
+
+    gpt2_pass(x, 0, Pn, 0, gen_len == 1)
+    P.mark("prefill_end")
+    for k in range(1, gen_len):
+        gpt2_pass(x_dec, Pn + k - 1, 1, k, k == gen_len - 1)
+        P.mark(f"decode{k}_end")
+    P.mark("end")
+    assert P.arena.size == 0, "generator plans reference the shared weight arena only"
+    pl = P.finish(io, meta=dict(B=B, L=L, P=Pn, lmax=lmax, gen_len=gen_len, n_layer=W.n_layer))
+    pl.arena = W.arena
+    return pl

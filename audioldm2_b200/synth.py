@@ -70,6 +70,48 @@ def vocoder_state_dict(cfg: dict, seed: int = 1236) -> Dict[str, torch.Tensor]:
     return sd
 
 
+def seqgen_state_dict(seed: int = 1237, n_layer: int = 12) -> Dict[str, torch.Tensor]:
+    """Seeded AudioMAE-generator checkpoint (keys relative to ``cond_stage_models.<i>.``).  Not ``_fill``: GPT-2's
+    ``Conv1D`` weights are [in, out], so their fan-in is ``shape[0]``; ``wpe`` / ``wte`` are 0.02 N(0, 1) (GPT-2's
+    embedding init) and the SOS / EOS tables N(0, 1) (the ``nn.Embedding`` default).  Everything else as SURVEY.md 8d."""
+    shapes = arch.seqgen_param_shapes(n_layer)
+    g = torch.Generator(device="cpu")
+    g.manual_seed(seed)
+    out = {}
+    for name in sorted(shapes):
+        shp = shapes[name]
+        t = torch.randn(shp, generator=g)
+        if name in ("model.wpe.weight", "model.wte.weight"):
+            t = 0.02 * t
+        elif name.endswith("_of_sequence_tokens.weight"):
+            pass
+        elif name.endswith(".bias"):
+            t = 0.02 * t
+        elif len(shp) == 1:
+            t = 1.0 + 0.1 * t
+        elif name.startswith("model."):                 # Conv1D [in, out]
+            t = t / math.sqrt(shp[0])
+        else:                                           # nn.Linear [out, in]
+            t = t / math.sqrt(shp[1])
+        out[name] = t.contiguous()
+    return out
+
+
+def encoder_outputs(batch: int, t5_lens, seed: int = 78, device="cpu"):
+    """Synthetic encoder outputs for the sequence-generation models (SURVEY.md 8d): CLAP [B, 1, 512] L2-normalised (as
+    the CLAP embedding is), Flan-T5 hidden states [B, L, 1024] N(0, 1) with L = max(t5_lens) and the padding mask of
+    per-row lengths ``t5_lens`` (zeros behind each row's length, as the tokenizer's padding=True gives)."""
+    g = torch.Generator(device="cpu"); g.manual_seed(seed)
+    lens = [int(n) for n in t5_lens]
+    assert len(lens) == batch and min(lens) >= 1
+    L = max(lens)
+    clap = torch.randn(batch, 1, 512, generator=g)
+    clap = clap / clap.norm(dim=-1, keepdim=True)
+    t5 = torch.randn(batch, L, 1024, generator=g)
+    mask = (torch.arange(L)[None, :] < torch.tensor(lens)[:, None]).float()
+    return clap.to(device), t5.to(device), mask.to(device)
+
+
 def conditioning(cfg: dict, batch: int, seed: int = 77, t5_len: int = 32, device="cpu"):
     """Synthetic conditioning at the UNet boundary (SURVEY.md 8d).
 

@@ -25,6 +25,9 @@
  *       models/ddpm.py:928-939, hifigan/models.py:149-165
  *   TacotronSTFT.mel_spectrogram                                 aldm_stft_mel
  *       utilities/audio/stft.py:159-178
+ *   SequenceGenAudioMAECond.forward -> Sequence2AudioMAE.generate aldm_program_run(seqgen program: GPT-2 prefill +
+ *       audiomae_gen/sequence_input.py:110-201,294-325,           7 KV-cached decode passes; ALDM_OP_SEQ_ASSEMBLE,
+ *       encoders/modules.py:271-300                                ALDM_OP_KV_ATTN, ALDM_OP_SEQ_FEEDBACK)
  *
  * Conventions
  *   - all pointers are DEVICE pointers unless named host_*; buffers are caller-owned (torch
@@ -48,7 +51,7 @@
 extern "C" {
 #endif
 
-#define ALDM_ABI_VERSION 8
+#define ALDM_ABI_VERSION 9
 #define ALDM_MAX_TAPS 16
 
 enum {
@@ -67,7 +70,8 @@ enum { ALDM_GEMM_TC = 0, ALDM_GEMM_SIMT = 1, ALDM_GEMM_TC_V1 = 2 };   /* aldm_ge
 /* OR-ed into aldm_gemm_desc.impl: w_packed is never written while the program runs (model weights), so the
  * kernel may start streaming it before its programmatic-dependency wait (overlapping the previous kernel's tail). */
 #define ALDM_GEMM_STATIC_B (1 << 16)
-enum { ALDM_ACT_NONE = 0, ALDM_ACT_GEGLU = 1, ALDM_ACT_TANH = 2, ALDM_ACT_SILU = 3 };
+/* ALDM_ACT_GELU_TANH: 0.5 v (1 + tanh(sqrt(2/pi) (v + 0.044715 v^3))), GPT-2's gelu_new (accurate tanhf) */
+enum { ALDM_ACT_NONE = 0, ALDM_ACT_GEGLU = 1, ALDM_ACT_TANH = 2, ALDM_ACT_SILU = 3, ALDM_ACT_GELU_TANH = 4 };
 enum { ALDM_OUT_F32 = 0, ALDM_OUT_PLANES = 1, ALDM_OUT_NCHW = 2, ALDM_OUT_QKV = 3 };
 
 /* out[row(m), n] = epilogue( sum_k A[m, k] * W[n, k] ),  k = tap * Cp + c
@@ -221,10 +225,55 @@ int aldm_posterior_sample(const float* moments, const float* noise_nchw, float* 
 int aldm_stft_mel(const float* wav, int32_t B, int32_t T, int32_t n_fft, int32_t hop,
                   const float* mel_basis, int32_t n_mels, float* out, int32_t out_frames, void* stream);
 
+/* ---- AudioMAE token generation: GPT-2 with a KV cache (csrc/cond/seqgen.cu) ------------------
+ * The sequence of one generator call is [sos0, clap, eos0, sos1, t5[0..L), eos1] (P = L + 5 positions) followed by the
+ * generated tokens.  Each GPT-2 layer keeps an fp32 sequence buffer seq[B, lmax, 3C] with one row of q | k | v per
+ * position, written in place by the c_attn GEMM through its output row mapping (OHF = lmax, ooy = first position).
+ * mask[B, lmax] holds 1 for the positions a query may attend to (the T5 padding holds 0); key 0 must be 1. */
+
+/* Causal attention, head_dim 64, queries at positions [p0, p0 + nq) of every batch row, keys [0, p0 + q] with
+ * mask[b, key] == 1; scale applied to q.k; fp32 softmax and accumulation.  Output: planes [B * nq, ldo], head h at
+ * columns [h*64, +64) (row b * nq + q).  lmax <= 1024, p0 + nq <= lmax. */
+typedef struct aldm_kv_attn_desc {
+  const float* seq;          /* [B, lmax, ld_seq]: q at columns [0, C), k at [C, 2C), v at [2C, 3C), C = heads * 64 */
+  const float* mask;         /* [B, lmax] */
+  void* out_hi; void* out_lo;
+  int32_t B, heads, lmax, ld_seq, p0, nq, ldo;
+  float scale;
+} aldm_kv_attn_desc;
+int aldm_kv_attention(const aldm_kv_attn_desc* d, void* stream);
+
+/* Prefill residual stream x[B * P, C], P = L + 5: rows 1 and [4, 4 + L) of every batch row already hold the CLAP and T5
+ * projections (written there by their GEMMs); rows 0, 2, 3, L + 4 become sos[0], eos[0], sos[1], eos[1]; then
+ * x[b, p] += wpe[p] for every p < P.  mask[B, lmax] = t5_mask at the T5 positions, 1 everywhere else (lmax >= P). */
+typedef struct aldm_seq_assemble_desc {
+  float* x;
+  const float* sos; const float* eos;     /* [>= 2, C] */
+  const float* wpe;                       /* [>= P, C] */
+  const float* t5_mask;                   /* [B, L] */
+  float* mask;                            /* [B, lmax] */
+  int32_t B, L, lmax, C;
+} aldm_seq_assemble_desc;
+int aldm_seq_assemble(const aldm_seq_assemble_desc* d, void* stream);
+
+/* Last position of every batch row (x row b * nq + nq - 1, at sequence position pos): y = ln_f(x) in fp32 (two-pass
+ * statistics); out[b, k, :] = y (out is [B, gen_len, C]); next[b, :] = y + wpe[pos + 1] unless next is NULL. */
+typedef struct aldm_seq_feedback_desc {
+  const float* x;
+  const float* gamma; const float* beta;
+  const float* wpe;
+  float* out;
+  float* next;
+  int32_t B, nq, C, pos, k, gen_len;
+  float eps;
+} aldm_seq_feedback_desc;
+int aldm_seq_feedback(const aldm_seq_feedback_desc* d, void* stream);
+
 /* ---- programs: flat op tables replayed on a stream / as a CUDA graph ---------------------- */
 
 enum { ALDM_OP_GEMM = 1, ALDM_OP_PREP = 2, ALDM_OP_ATTN = 3, ALDM_OP_SOFTMAX = 4, ALDM_OP_TEMB = 5,
-       ALDM_OP_TRANSPOSE = 6, ALDM_OP_PACKB = 7, ALDM_OP_COPY = 8 };
+       ALDM_OP_TRANSPOSE = 6, ALDM_OP_PACKB = 7, ALDM_OP_COPY = 8, ALDM_OP_SEQ_ASSEMBLE = 9, ALDM_OP_KV_ATTN = 10,
+       ALDM_OP_SEQ_FEEDBACK = 11 };
 
 typedef struct aldm_op {
   int32_t kind;
@@ -238,6 +287,9 @@ typedef struct aldm_op {
     struct { const float* src; float* dst; int32_t B, C, HW, to_nhwc; } transpose;
     struct { const float* src; void* dst_packed; float* dst_plain; int32_t lds, transpose, N, K, bn; } packb;
     struct { const void* src; void* dst; int64_t bytes; } copy;
+    aldm_seq_assemble_desc seq_assemble;
+    aldm_kv_attn_desc kv_attn;
+    aldm_seq_feedback_desc seq_feedback;
   } u;
 } aldm_op;
 
