@@ -10,13 +10,16 @@
 // (SURVEY.md 7 H1: plain single-pass bf16 / TF32-class rounding of BOTH operands misses or crowds the 1e-3 waveform
 // tolerance; rounding only the activations to 11 bits costs 2e-4 at 200 steps.)
 //
-// Structure of one CTA (persistent: 416 threads, one CTA per SM looping over 128 x BN output tiles / split-K slices):
-//   warps 0-7   two consumer warpgroups: wgmma on 64-row halves of the tile, then the epilogue of the tile from an fp32
-//               copy of the accumulator in shared memory.
-//   warps 8-11  A producers: gather 16-byte chunks (8 channels of one tap of one pixel) with cp.async + zero fill into
+// Structure of one CTA (persistent: 512 threads = four warpgroups, one CTA per SM looping over 128 x BN output tiles /
+// split-K slices):
+//   warps 0-7   two consumer warpgroups: wgmma on 64-row halves of the tile, then the accumulator is handed to the
+//               epilogue warpgroup as an fp32 tile in shared memory and the consumers go on to the next tile.
+//   warps 8-11  producers: gather A in 16-byte chunks (8 channels of one tap of one pixel) with cp.async + zero fill into
 //               128B-swizzled K-major tiles; completion is signalled on the stage's mbarrier (cp.async.mbarrier.arrive).
-//   warp 12     B producer: one ELECTED lane (elect.sync) issues a TMA bulk copy (cp.async.bulk) of the host-packed,
+//               One ELECTED lane (elect.sync) of warp 8 also issues a TMA bulk copy (cp.async.bulk) of the host-packed,
 //               pre-swizzled weight tile image (hi|lo) per stage.
+//   warps 12-15 epilogue warpgroup: warp w finishes rows [32 w, 32 w + 32) of the tile, all BN columns, while the
+//               consumers already run the next tile's MMAs.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -282,30 +285,30 @@ __device__ __forceinline__ void emit_rows(const aldm_gemm_desc& d, const CR& cr,
   __syncwarp();
 }
 
-// ---- full-line finish for single-plane fp16 outputs (EPI_PLN, EPI_GEGLU -> planes) ------------------------
-// A warp's 32 x 32 chunk is only 64 bytes per row in fp16: stored by itself it is a stream of half-line transactions, and the
+// ---- full-line finish for single-plane fp16 outputs (EPI_PLN, EPI_GEGLU -> planes, Q|K planes) --------------------------
+// A 32 x 32 chunk is only 64 bytes per row in fp16: stored by itself it is a stream of half-line transactions, and the
 // SM's store port moves one transaction per clock whatever its size (scripts/store_rate.py measures it), so half-line
-// stores halve the store bandwidth of the epilogue.  The two warps that own the same accumulator row quarter
-// (chunk parity 0 / 1: columns [0,32) and [32,64) of one 64-column group) therefore assemble the 32 x 64 fp16 block in a shared
-// tile (rows of 128 bytes, 16-byte chunks XOR-swizzled by the row), meet at a 64-thread named barrier, and each stores 16
-// complete 128-byte rows: 4 STG.128 per warp instead of 8 STG.64.  Two tiles alternate, so one barrier per block suffices.
-template <typename CR>
-__device__ __forceinline__ void emit_pair_hi(const aldm_gemm_desc& d, const CR& cr, int n_pair0, uint8_t* tile, int lane, int half,
-                                             int bar_id, const float* v) {
+// stores halve the store bandwidth of the epilogue.  The warp therefore packs the two 32-column chunks of one 64-column
+// group (part 0 / 1) into its staging tile (rows of 128 bytes, 16-byte chunks XOR-swizzled by the row) and then stores the
+// 32 x 64 fp16 block as 32 complete 128-byte rows: 8 STG.128 per block instead of 16 STG.64.
+__device__ __forceinline__ void line_put_hi(uint8_t* tile, int lane, int part, const float* v) {
   uint8_t* wr = tile + lane * 128;
   const int sw = lane & 7;
 #pragma unroll
-  for (int j = 0; j < 4; ++j) *reinterpret_cast<uint4*>(wr + (((half * 4 + j) ^ sw) << 4)) = pack8_hi(v + 8 * j);
-  asm volatile("bar.sync %0, 64;" ::"r"(bar_id) : "memory");
+  for (int j = 0; j < 4; ++j) *reinterpret_cast<uint4*>(wr + (((part * 4 + j) ^ sw) << 4)) = pack8_hi(v + 8 * j);
+}
+template <typename CR>
+__device__ __forceinline__ void line_store_hi(const aldm_gemm_desc& d, const CR& cr, int n_group0, const uint8_t* tile, int lane) {
+  __syncwarp();
   const int rs = lane >> 3, c8 = lane & 7;
   aldm_plane_t* out = reinterpret_cast<aldm_plane_t*>(d.out_hi);
 #pragma unroll
-  for (int it = 0; it < 4; ++it) {
-    const int rr = half * 16 + it * 4 + rs;
+  for (int it = 0; it < 8; ++it) {
+    const int rr = it * 4 + rs;
     const uint4 x = *reinterpret_cast<const uint4*>(tile + rr * 128 + ((c8 ^ (rr & 7)) << 4));
-    const auto orow = half ? cr.orow[4 + it] : cr.orow[it];
-    if ((cr.vmask >> rr) & 1u) *reinterpret_cast<uint4*>(out + (orow * d.ldo + n_pair0 + c8 * 8)) = x;
+    if ((cr.vmask >> rr) & 1u) *reinterpret_cast<uint4*>(out + (cr.orow[it] * d.ldo + n_group0 + c8 * 8)) = x;
   }
+  __syncwarp();
 }
 
 // ------------------------------------------------------------------------------------------
@@ -320,10 +323,10 @@ struct Tc3Cfg {
   static constexpr int STAGE_BYTES = AP * A_BYTES + 2 * B_BYTES;      // [a_hi | a_lo (AP == 2)] [b_hi | b_lo]
   static constexpr int B_OFF = AP * A_BYTES;
   static constexpr int ACC_BYTES = BM * BN * 4;       // fp32 accumulator tile handed from the warpgroups to the epilogue
-  static constexpr int STG_BYTES = 8 * 32 * 33 * 4;   // one 32x33 fp32 transpose tile per epilogue warp
+  static constexpr int STG_BYTES = 4 * 32 * 33 * 4;   // one 32x33 fp32 transpose tile per epilogue warp
   static constexpr int SMEM_MAX = 227 * 1024;
   static constexpr int FIT = (SMEM_MAX - 1024 - 256 - STG_BYTES - ACC_BYTES) / STAGE_BYTES;
-  static constexpr int STAGES = FIT > 4 ? 4 : FIT;    // BN=128: 2 stages; BN=64: 3; BN=32: 4
+  static constexpr int STAGES = FIT > 4 ? 4 : FIT;    // BN=128: 2 stages (AP 2) / 3 (AP 1); BN=64: 3 / 4; BN=32: 4
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + STG_BYTES;
   static_assert(STAGES >= 2, "pipeline needs two stages");
   static_assert(SMEM_BYTES <= SMEM_MAX, "shared memory");
@@ -354,7 +357,16 @@ __device__ __forceinline__ void acc_ld32(const float* accb, int row, int c0, uin
     r[4 * j + 2] = __float_as_uint(x.z); r[4 * j + 3] = __float_as_uint(x.w);
   }
 }
-__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// Register split of the persistent kernel (setmaxnreg, per thread).  Its four warpgroups put one warp of each role on
+// every scheduler sub-partition: 80 (producer) + 2 x 136 (consumers) + 160 (epilogue) = 512 registers x 32 lanes, the
+// sub-partition's 16,384.  The kernel is compiled for 512 threads at 128 registers, which is the same total.  80 is the
+// least that holds the producers' per-row state without spilling; no instance spills at this split (ptxas -v).
+constexpr int kProdRegs = 80, kConsRegs = 136, kEpiRegs = 160;
+static_assert(kProdRegs + 2 * kConsRegs + kEpiRegs == 4 * 128, "register split must use exactly the launch allocation");
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // Debug timeline (profiling aid, dbg bit 128): CTA 0 records clock64() at pipeline events.
 // layout: [role 0..3][iteration 0..255][phase 0..1]
@@ -365,12 +377,17 @@ __device__ long long g_timeline[4 * 256 * 2];
   } while (0)
 
 // ------------------------------------------------------------------------------------------
-// persistent variant (default): one CTA per SM loops over output tiles; 416 threads =
-//   warps 0-7 two consumer warpgroups (wgmma into register accumulators, rows [64 wg, 64 wg + 64) of the tile),
-//   then the epilogue of the same tile | warps 8-11 A producers | warp 12 B (TMA bulk).
-// The finished accumulator is staged in shared memory (fp32, 16-byte chunks swizzled by row) so that each epilogue
-// warp reads whole rows: warp ew owns rows [32 (ew & 3), +32) and alternates 32-column chunks with warp ew ^ 4.
-// While the consumers run the epilogue, the producers already fill the pipeline with the next tile's stages.
+// persistent variant (default): one CTA per SM loops over output tiles; 512 threads = four warpgroups:
+//   WG0, WG1 (warps 0-7)   consumers: wgmma into register accumulators, rows [64 wg, 64 wg + 64) of the tile;
+//   WG2      (warps 8-11)  producers: the A gather, and the weight TMA from one elected lane of warp 8;
+//   WG3      (warps 12-15) epilogue: warp ew finishes rows [32 ew, 32 ew + 32) of the tile, all BN columns.
+// Accumulator hand-off, one 64 KB fp32 tile in shared memory (16-byte chunks swizzled by row, so that each epilogue lane
+// reads a whole row) and two mbarriers that both complete once per tile, so that their phase is the parity of the CTA's
+// tile counter: after the main loop of tile t the consumers wait acc_empty (the epilogue of t-1 is done reading the
+// buffer), store the accumulator, arrive acc_full (one arrival per consumer warp) and start tile t+1.  The epilogue
+// warpgroup walks the same tile sequence: it decodes the rows and fetches bias / residual of tile t, waits acc_full,
+// finishes the tile and arrives acc_empty (one arrival per warp).  One buffer is enough: the consumers only need it
+// again after a whole main loop, and the epilogue of tile t runs under the MMAs of tile t+1.
 // The producers' per-stage work is one add + one bit test per row: row bases and per-row tap-validity masks are
 // computed once per tile.  EPI selects a specialised epilogue body at compile time (0: linear/conv with optional
 // bias, row vector, residual, dual/QKV plane outputs; 1: GEGLU; 2: everything else; 3/4: compact fp32 / planes).
@@ -410,7 +427,7 @@ struct Tc3Divs {
 
 // AP = number of A planes (2: hi + lo, three MMAs per K step; 1: hi only, two MMAs and half the A bytes).
 template <int BN, int EPI, int AP>
-__global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant__ aldm_gemm_desc d, int tiles_m, int tiles_n,
+__global__ void __launch_bounds__(512, 1) gemm_tc3_kernel(const __grid_constant__ aldm_gemm_desc d, int tiles_m, int tiles_n,
                                                            const __grid_constant__ Tc3Divs fd) {
   using C = Tc3Cfg<BN, AP>;
   extern __shared__ uint8_t smem_raw[];
@@ -420,6 +437,8 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
   const uint32_t bar_base = acc_base + C::ACC_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
+  const uint32_t acc_full = bar_base + 8u * (2 * C::STAGES);
+  const uint32_t acc_empty = acc_full + 8u;
   float* accb = reinterpret_cast<float*>(smem_raw + (acc_base - raw));
 
   const int tid = threadIdx.x;
@@ -435,13 +454,14 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
       mbar_init(full_bar(s), 128 + 1);   // 128 cp.async producers (completion-triggered arrivals) + B expect_tx
       mbar_init(empty_bar(s), 8);        // one arrival per consumer warp once its MMAs on the stage have completed
     }
+    mbar_init(acc_full, 8);              // one arrival per consumer warp: its rows of the accumulator are in shared memory
+    mbar_init(acc_empty, 4);             // one arrival per epilogue warp: done reading the accumulator tile
     fence_barrier_init();
   }
   __syncthreads();
-  // Everything above overlapped the predecessor's tail; nothing below may touch its outputs before the wait.
-  // The weight stream is the exception (ALDM_GEMM_STATIC_B): warp 12 starts filling the pipeline right away.
-  // The A producers wait inside their branch, after the (memory-free) row decode of their first tile.
-  if (warp < 8 || (warp == 12 && !(d.impl & ALDM_GEMM_STATIC_B))) pdl_wait();
+  // Everything above overlapped the predecessor's tail; nothing below may touch its outputs before the wait.  Each role
+  // waits inside its branch: the producers after the (memory-free) row decode of their first tile, and after the first
+  // weight stages when those do not depend on the predecessor (ALDM_GEMM_STATIC_B).
 
   auto tile_coords = [&](int id, int& mt, int& nt, int& z, int& kb0, int& nkb) {
     int r = id;
@@ -456,7 +476,8 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
   };
 
   if (warp >= 8 && warp < 12) {
-    // ===================== A producers =====================
+    // ===================== producers: A gather + weight TMA =====================
+    setmaxnreg_dec<kProdRegs>();
     const int ptid = tid - 256;
     const int j = ptid & 7;                 // 16-byte chunk (8 channels) inside the 64-wide K block
     const int rbase = ptid >> 3;            // rows rbase + 16*i
@@ -466,9 +487,10 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
     const aldm_plane_t* alo = reinterpret_cast<const aldm_plane_t*>(d.a_lo);
     uint32_t cnt = 0;
     int last_mt = -1;
-    int rowoff[8];            // element offset of tap (0,0) / channel 0 of each row (valid rows only)
+    // Per-row state, kept small: the producers run at kProdRegs registers.
+    int rowoff[8];            // element offset of tap (0,0) / channel 0 of each row (valid rows only); up = 1: b * Hs
     uint32_t tapmask[8];      // bit (t + 4) set <=> tap t of this row is inside the input (pre-shifted: (mask >> t) & 16 = bytes to copy)
-    int ih0[8], iw0[8], pbh[8];   // only used by the nearest-upsample (up = 1) slow path
+    uint32_t yx0[8];          // up = 1 only: first input row | column << 16 (before the nearest-upsample shift)
     // Row decode of one M tile.  A single warp per scheduler runs this dependent integer chain slowly and the tensor
     // core idles meanwhile at every tile boundary of the short-K linear layers: linear layers take the trivial branch,
     // and the first tile is decoded before the programmatic-dependency wait (under the previous kernel's tail).
@@ -476,9 +498,8 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int m = mt * C::BM + rbase + 16 * i;
-        uint32_t msk = 0;
+        uint32_t msk = 0, yx = 0;
         int off = 0;
-        ih0[i] = 0; iw0[i] = 0; pbh[i] = -1;
         if (fd.plain) {
           if (m < M) { msk = 16u; off = m * d.Cp; }
         } else if (m < M) {
@@ -489,22 +510,39 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
           int bs = b;
           if (d.bmod > 0) { int q; fd.bmod.divmod(b, q, bs); }
           const int pb = bs * Hs;
-          ih0[i] = y0; iw0[i] = x0; pbh[i] = pb;
+          yx = (uint32_t)y0 | ((uint32_t)x0 << 16);
           for (int tp = 0; tp < d.ntaps; ++tp) {
             const int ih = y0 + d.dy[tp], iw = x0 + d.dx[tp];
             if (ih >= 0 && ih < d.H && iw >= 0 && iw < d.W) msk |= 16u << tp;
           }
-          off = ((pb + y0) * Ws + x0) * d.Cp;
+          off = d.up ? pb : ((pb + y0) * Ws + x0) * d.Cp;
         }
         tapmask[i] = msk;
         rowoff[i] = off;
+        yx0[i] = yx;
       }
     };
+    // The weight tile of every stage: one elected lane of warp 8 issues the bulk copy after the same empty-slot wait.
+    const bool b_lane = warp == 8 && elect_one();
+    auto w_tile = [&](int nt, int kb0) {
+      return reinterpret_cast<const uint8_t*>(d.w_packed) + ((long long)nt * nkb_total + kb0) * (2 * C::B_BYTES);
+    };
+    auto issue_b = [&](uint32_t n, int s, const uint8_t* src) {
+      ALDM_TL(1, n, 0);
+      if (dbg & 2) { mbar_arrive(full_bar(s)); return; }
+      mbar_arrive_expect_tx(full_bar(s), 2 * C::B_BYTES);
+      bulk_g2s(base + s * C::STAGE_BYTES + C::B_OFF, src, 2 * C::B_BYTES, full_bar(s));
+    };
+    uint32_t b_pre = 0;       // weight stages issued before the dependency wait
     if ((int)blockIdx.x < total) {
       int mt, nt, z, kb0, nkb;
       tile_coords(blockIdx.x, mt, nt, z, kb0, nkb);
       decode_rows(mt);
       last_mt = mt;
+      if (b_lane && (d.impl & ALDM_GEMM_STATIC_B)) {     // the weights do not depend on the predecessor: fill the free stages now
+        b_pre = (uint32_t)(nkb < C::STAGES ? nkb : C::STAGES);
+        for (uint32_t it = 0; it < b_pre; ++it) issue_b(it, (int)it, w_tile(nt, kb0) + (long long)it * (2 * C::B_BYTES));
+      }
     }
     pdl_wait();
     for (int id = blockIdx.x; id < total; id += gridDim.x) {
@@ -514,6 +552,7 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
         last_mt = mt;
         decode_rows(mt);
       }
+      const uint8_t* wsrc = w_tile(nt, kb0);
       // (tap, c) of this thread's 8-channel chunk at the first k-block of the tile, then advanced by 64 per block
       const int k = kb0 * C::BK + j * 8;
       int tap, c;
@@ -522,6 +561,7 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
         const int s = cnt % C::STAGES;
         mbar_wait(empty_bar(s), ((cnt / C::STAGES) & 1) ^ 1);
         if (ptid == 0) ALDM_TL(0, cnt, 0);
+        if (b_lane && cnt >= b_pre) issue_b(cnt, s, wsrc + (long long)it * (2 * C::B_BYTES));
         const bool kvalid = tap < d.ntaps;
         const int tp = kvalid ? tap : 0;
         const uint32_t sa = base + s * C::STAGE_BYTES + swz;
@@ -567,7 +607,8 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
           for (int i = 0; i < 8; ++i) {
             const bool ok = kvalid && ((tapmask[i] >> (tp + 4)) & 1u);
             long long off = 0;
-            if (ok) off = ((long long)(pbh[i] + ((ih0[i] + dy) >> 1)) * Ws + ((iw0[i] + dx) >> 1)) * d.Cp + c;
+            const int ih = (int)(yx0[i] & 0xffffu) + dy, iw = (int)(yx0[i] >> 16) + dx;
+            if (ok) off = ((long long)(rowoff[i] + (ih >> 1)) * Ws + (iw >> 1)) * d.Cp + c;
             const uint32_t dst = sa + (uint32_t)(rbase + 16 * i) * 128u;
             cp_async_16(dst, ahi + off, ok ? 16u : 0u);
             if (AP == 2) cp_async_16(dst + C::A_BYTES, alo + off, ok ? 16u : 0u);
@@ -579,40 +620,17 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
         while (c >= d.Cp) { c -= d.Cp; ++tap; }
       }
     }
-  } else if (warp == 12) {
-    // ===================== B producer =====================
-    if (elect_one()) {
-      uint32_t cnt = 0;
-      for (int id = blockIdx.x; id < total; id += gridDim.x) {
-        int mt, nt, z, kb0, nkb;
-        tile_coords(id, mt, nt, z, kb0, nkb);
-        const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(d.w_packed) + ((long long)nt * nkb_total + kb0) * (2 * C::B_BYTES);
-        for (int it = 0; it < nkb; ++it, ++cnt) {
-          const int s = cnt % C::STAGES;
-          mbar_wait(empty_bar(s), ((cnt / C::STAGES) & 1) ^ 1);
-          ALDM_TL(1, cnt, 0);
-          if (dbg & 2) { mbar_arrive(full_bar(s)); continue; }
-          mbar_arrive_expect_tx(full_bar(s), 2 * C::B_BYTES);
-          bulk_g2s(base + s * C::STAGE_BYTES + C::B_OFF, wsrc + (long long)it * (2 * C::B_BYTES), 2 * C::B_BYTES,
-                   full_bar(s));
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================== consumers: warpgroup wg = rows [64 wg, 64 wg + 64) of the tile; then the epilogue =====================
+  } else if (warp < 8) {
+    // ===================== consumers: warpgroup wg = rows [64 wg, 64 wg + 64) of the tile =====================
+    setmaxnreg_inc<kConsRegs>();
+    pdl_wait();
     const int wg = warp >> 2;
-    const int ew = warp;                 // epilogue role: rows [32 lb, 32 lb + 32), chunk parity `half`
-    const int lb = ew & 3;
-    const int half = ew >> 2;
-    const int trow_in_tile = lb * 32 + lane;
-    float* stg = reinterpret_cast<float*>(smem_raw + (bar_base + 256 - raw)) + ew * (32 * 33);
-    uint32_t cnt = 0, tl = 0, pair_cnt = 0;
+    uint32_t cnt = 0, tl = 0;
     float acc[BN / 2];
     for (int id = blockIdx.x; id < total; id += gridDim.x, ++tl) {
       int mt, nt, z, kb0, nkb;
       tile_coords(id, mt, nt, z, kb0, nkb);
-      // (the asm operands are read-write: a defined start value keeps the accumulator dead during the epilogue)
+      // (the asm operands are read-write: a defined start value keeps the accumulator dead between tiles)
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       for (int it = 0; it < nkb; ++it, ++cnt) {
@@ -645,6 +663,33 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
       if (lane == 0) mbar_arrive(empty_bar((cnt - 1) % C::STAGES));
       // all MMAs of this CTA are done: let the next kernel's blocks be scheduled under the last epilogue
       if (tid == 0 && id + (int)gridDim.x >= total) pdl_launch();
+      // hand the accumulator over once the epilogue is done reading the previous tile's
+      mbar_wait(acc_empty, (tl & 1) ^ 1);
+      acc_st_frag<BN>(accb, wg * 64 + (warp & 3) * 16, lane, acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(acc_full);
+    }
+  } else {
+    // ===================== epilogue: warp ew = rows [32 ew, 32 ew + 32) of the tile, all BN columns =====================
+    setmaxnreg_inc<kEpiRegs>();
+    pdl_wait();
+    const int ew = warp - 12;
+    const int trow_in_tile = ew * 32 + lane;
+    float* stg = reinterpret_cast<float*>(smem_raw + (bar_base + 256 - raw)) + ew * (32 * 33);
+    uint8_t* stg8 = reinterpret_cast<uint8_t*>(stg);
+    constexpr bool kCompact = EPI == EPI_F32N || EPI == EPI_PLN;
+    constexpr int NCH = BN / 32;              // 32-column chunks per row
+    constexpr int NRV = NCH > 1 ? 2 : 1;      // residual prefetch buffers (rotating)
+    constexpr int NGV = BN >= 64 ? BN / 64 : 1;   // GEGLU: 32-column value chunks per row
+    // full-line stores (line_store_hi): single fp16 plane out, no residual, whole 64-column groups (conditions: gemm_select)
+    const bool pair_pln = EPI == EPI_PLN && BN >= 64 && fd.store == ALDM_STORE_PAIR_PLN;
+    const bool pair_geglu = EPI == EPI_GEGLU && BN == 128 && fd.store == ALDM_STORE_PAIR_GEGLU;
+    const bool pair_qk = EPI == EPI_FAST && BN >= 64 && fd.store == ALDM_STORE_PAIR_QK;
+    const bool has_res = kCompact && d.res != nullptr;
+    uint32_t tl = 0;
+    for (int id = blockIdx.x; id < total; id += gridDim.x, ++tl) {
+      int mt, nt, z, kb0, nkb;
+      tile_coords(id, mt, nt, z, kb0, nkb);
       const int m = mt * C::BM + trow_in_tile;
       RowInfo r;
       {
@@ -655,50 +700,38 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
         fd.oh.divmod(t, r.b, r.oh);
         r.orow = ((long long)r.b * d.OHF + (long long)r.oh * d.osy + d.ooy) * d.OWF + r.ow;
       }
-      constexpr bool kCompact = EPI == EPI_F32N || EPI == EPI_PLN;
       CoRows cr;
       CoRows32 cr32;
       if (kCompact) cr32 = co_rows32(r, lane); else cr = co_rows(r, lane);
-      // compact epilogues: bias and the first chunk's residual are fetched while the tile is still being accumulated
-      constexpr int NCH = (BN + 63) / 64;       // 32-column chunks per epilogue warp
-      constexpr int NRV = NCH > 1 ? 2 : 1;      // residual prefetch buffers (rotating)
-      uint8_t* stg8 = reinterpret_cast<uint8_t*>(stg);
+      // bias and the first residual chunks are fetched while the consumers still accumulate the tile
       float4 pb4[NCH], prv[NRV][8];
-      const bool has_res = kCompact && d.res != nullptr;
-      if (kCompact && d.splitk == 1) {
+      if (kCompact) {
 #pragma unroll
         for (int ch = 0; ch < NCH; ++ch) {
-          const int n = nt * BN + half * 32 + 64 * ch + (lane & 7) * 4;
+          const int n = nt * BN + 32 * ch + (lane & 7) * 4;
           pb4[ch] = (d.bias && n < d.N) ? __ldg(reinterpret_cast<const float4*>(d.bias + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
-        // BOTH chunks' residuals are requested here, before the accumulator is staged: issued after the first chunk was
-        // staged, the loads would queue behind that chunk's stores in the LSU and the second chunk would wait for them.
 #pragma unroll
         for (int ch = 0; ch < NRV; ++ch)
-          if (has_res && half * 32 + 64 * ch < BN) co_load_res32(d, cr32, nt * BN + half * 32 + 64 * ch, d.N, lane, prv[ch]);
+          if (has_res) co_load_res32(d, cr32, nt * BN + 32 * ch, d.N, lane, prv[ch]);
       }
-      // full-line pair mode (emit_pair_hi): single fp16 plane out, no residual, whole 64-column groups (conditions: gemm_select)
-      const bool pair_pln = EPI == EPI_PLN && BN >= 64 && fd.store == ALDM_STORE_PAIR_PLN;
-      const bool pair_geglu = EPI == EPI_GEGLU && BN == 128 && fd.store == ALDM_STORE_PAIR_GEGLU;
-      const bool pair_qk = EPI == EPI_FAST && BN >= 64 && fd.store == ALDM_STORE_PAIR_QK;
-      uint8_t* pair_tiles = reinterpret_cast<uint8_t*>(smem_raw + (bar_base + 256 - raw)) + (ew & 3) * (32 * 33 * 4);
-      const int pair_bar = 1 + (ew & 3);
-      float pln_b[NCH > 0 ? NCH : 1];      // bias of this warp's columns (lane = column), distributed by shuffles in pair mode
+      float pln_b[NCH];      // bias of each chunk's columns (lane = column), distributed by shuffles in full-line mode
 #pragma unroll
       for (int ch = 0; ch < NCH; ++ch) {
-        const int n = nt * BN + half * 32 + 64 * ch + lane;
+        const int n = nt * BN + 32 * ch + lane;
         pln_b[ch] = (pair_pln && d.bias && n < d.N) ? __ldg(d.bias + n) : 0.f;
       }
-      float gb_v = 0.f, gb_g = 0.f;       // GEGLU bias of this warp's value / gate chunk (lane = column)
-      if (EPI == EPI_GEGLU && d.bias && d.splitk == 1 && half * 32 < BN / 2) {
-        gb_v = __ldg(d.bias + nt * BN + half * 32 + lane);
-        gb_g = __ldg(d.bias + nt * BN + BN / 2 + half * 32 + lane);
+      float gb_v[NGV], gb_g[NGV];       // GEGLU bias of each value / gate chunk (lane = column)
+#pragma unroll
+      for (int c = 0; c < NGV; ++c) {
+        gb_v[c] = 0.f; gb_g[c] = 0.f;
+        if (EPI == EPI_GEGLU && d.bias && d.splitk == 1) {
+          gb_v[c] = __ldg(d.bias + nt * BN + 32 * c + lane);
+          gb_g[c] = __ldg(d.bias + nt * BN + BN / 2 + 32 * c + lane);
+        }
       }
       if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8, 0);      // tile prologue (row decode, bias / residual prefetch) done
-      // stage the accumulator tile in shared memory, once every warp is done reading the previous tile's
-      named_bar_sync(5, 256);
-      acc_st_frag<BN>(accb, wg * 64 + (warp & 3) * 16, lane, acc);
-      named_bar_sync(5, 256);
+      mbar_wait(acc_full, tl & 1);
       if (ew == 0 && lane == 0) ALDM_TL(3, tl, 0);
       if (dbg & 8) {
         // skip
@@ -707,7 +740,7 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
         const int Mpad = tiles_m * C::BM, Npad = tiles_n * BN;
         const int rs = lane >> 3, c4 = (lane & 7) * 4;
 #pragma unroll 1
-        for (int c0 = half * 32; c0 < BN; c0 += 64) {
+        for (int c0 = 0; c0 < BN; c0 += 32) {
           uint32_t v[32];
           acc_ld32<BN>(accb, trow_in_tile, c0, v);
 #pragma unroll
@@ -716,45 +749,42 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
 #pragma unroll
           for (int it = 0; it < 8; ++it) {
             const int rr = it * 4 + rs;
-            float* wp = d.ws + ((long long)z * Mpad + mt * C::BM + lb * 32 + rr) * Npad + nt * BN + c0 + c4;
+            float* wp = d.ws + ((long long)z * Mpad + mt * C::BM + ew * 32 + rr) * Npad + nt * BN + c0 + c4;
             *reinterpret_cast<float4*>(wp) = make_float4(stg[rr * 33 + c4], stg[rr * 33 + c4 + 1], stg[rr * 33 + c4 + 2], stg[rr * 33 + c4 + 3]);
           }
           __syncwarp();
         }
       } else if (EPI == EPI_GEGLU) {
-        // tile columns [0,BN/2) values, [BN/2,BN) gates; output width N/2, coalescable and without residual
-        // (both checked on the host; the residual-free body keeps v/g in registers under the 128-register cap)
+        // tile columns [0,BN/2) values, [BN/2,BN) gates; output width N/2, coalescable and without residual (host-checked)
         const int n_out = d.N / 2;
         float4 rv[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) rv[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 1
-        for (int c0 = half * 32; c0 < BN / 2; c0 += 64) {
+#pragma unroll      // full unroll: the bias registers gb_v / gb_g are indexed by the chunk
+        for (int c = 0; c < NGV; ++c) {
+          const int c0 = 32 * c;
           const int n0 = nt * (BN / 2) + c0;
           uint32_t vr[32], gr[32];
           acc_ld32<BN>(accb, trow_in_tile, c0, vr);
           acc_ld32<BN>(accb, trow_in_tile, BN / 2 + c0, gr);
-          if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1, 0);
+          if (c == 0 && ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1, 0);
           float* v = reinterpret_cast<float*>(vr);
           float* g = reinterpret_cast<float*>(gr);
-          // bias: fetched (one coalesced load per warp) BEFORE the accumulator wait, distributed by shuffles -- the broadcast
-          // float4 loads it replaces sat between the accumulator read and the GELU with a full L2 round trip exposed
+          // bias: fetched (one coalesced load per warp) BEFORE the accumulator wait, distributed by shuffles
 #pragma unroll
           for (int i = 0; i < 32; ++i) {
-            v[i] += __shfl_sync(0xffffffffu, gb_v, i);
-            g[i] += __shfl_sync(0xffffffffu, gb_g, i);
+            v[i] += __shfl_sync(0xffffffffu, gb_v[c], i);
+            g[i] += __shfl_sync(0xffffffffu, gb_g[c], i);
           }
 #pragma unroll      // full unroll: v/g must stay in registers (a partial unroll indexes them dynamically -> local memory)
           for (int i = 0; i < 32; i += 8) geglu_mul<8>(v + i, g + i);
-          if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1, 1);
-          if (pair_geglu) {                         // the FF1 case: one fp16 plane for FF2, stored as full lines by the warp pair
-            emit_pair_hi(d, cr, nt * (BN / 2), pair_tiles + ((pair_cnt++ & 1u) ? 4 * (32 * 33 * 4) : 0), lane, half, pair_bar, v);
-            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2, 1);
+          if (c == 0 && ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1, 1);
+          if (pair_geglu) {                         // the FF1 case: one fp16 plane for FF2, stored as full lines
+            line_put_hi(stg8, lane, c & 1, v);
+            if (c & 1) line_store_hi(d, cr, nt * (BN / 2), stg8, lane);
           } else if (d.out_mode == ALDM_OUT_PLANES) {
             stage_rows(stg8, lane, v);
-            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2, 0);
             emit_rows<true>(d, cr, n0, n_out, stg8, lane, rv, false, make_float4(0.f, 0.f, 0.f, 0.f));
-            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2, 1);
           } else {
             epi_finish_coalesced(d, cr, n0, v, n_out, stg, lane, rv, false);
           }
@@ -762,37 +792,38 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
       } else if (kCompact && pair_pln) {
 #pragma unroll
         for (int ch = 0; ch < NCH; ++ch) {
-          const int c0 = half * 32 + 64 * ch;      // < BN: BN >= 64 in pair mode
           uint32_t vr[32];
-          acc_ld32<BN>(accb, trow_in_tile, c0, vr);
+          acc_ld32<BN>(accb, trow_in_tile, 32 * ch, vr);
           float* v = reinterpret_cast<float*>(vr);
           if (d.bias) {
 #pragma unroll
             for (int i = 0; i < 32; ++i) v[i] += __shfl_sync(0xffffffffu, pln_b[ch], i);
           }
-          emit_pair_hi(d, cr32, nt * BN + 64 * ch, pair_tiles + ((pair_cnt++ & 1u) ? 4 * (32 * 33 * 4) : 0), lane, half, pair_bar, v);
+          line_put_hi(stg8, lane, ch & 1, v);
+          if (ch & 1) line_store_hi(d, cr32, nt * BN + 64 * (ch >> 1), stg8, lane);
         }
       } else if (kCompact) {
 #pragma unroll
         for (int ch = 0; ch < NCH; ++ch) {
-          const int c0 = half * 32 + 64 * ch;
-          if (c0 < BN) {
-            const int n0 = nt * BN + c0;
-            uint32_t vr[32];
-            acc_ld32<BN>(accb, trow_in_tile, c0, vr);
-            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1 + 2 * ch, 0);
-            stage_rows(stg8, lane, reinterpret_cast<const float*>(vr));
-            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 1 + 2 * ch, 1);
-            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2 + 2 * ch, 0);
-            emit_rows<EPI == EPI_PLN>(d, cr32, n0, d.N, stg8, lane, prv[ch % NRV], has_res, pb4[ch]);
-            if (ew == 0 && lane == 0) ALDM_TL(3, 64 + tl * 8 + 2 + 2 * ch, 1);
-          }
+          const int c0 = 32 * ch;
+          const int n0 = nt * BN + c0;
+          const bool tl_on = ch < 2 && ew == 0 && lane == 0;
+          uint32_t vr[32];
+          acc_ld32<BN>(accb, trow_in_tile, c0, vr);
+          if (tl_on) ALDM_TL(3, 64 + tl * 8 + 1 + 2 * ch, 0);
+          stage_rows(stg8, lane, reinterpret_cast<const float*>(vr));
+          if (tl_on) ALDM_TL(3, 64 + tl * 8 + 1 + 2 * ch, 1);
+          if (tl_on) ALDM_TL(3, 64 + tl * 8 + 2 + 2 * ch, 0);
+          emit_rows<EPI == EPI_PLN>(d, cr32, n0, d.N, stg8, lane, prv[ch % NRV], has_res, pb4[ch]);
+          if (tl_on) ALDM_TL(3, 64 + tl * 8 + 2 + 2 * ch, 1);
+          // the buffer just consumed takes the residual of the chunk NRV ahead
+          if (has_res && ch + NRV < NCH) co_load_res32(d, cr32, n0 + 32 * NRV, d.N, lane, prv[ch % NRV]);
         }
       } else if (EPI == EPI_FAST) {
         // no activation; fp32 / planes / dual / QKV outputs, all through the coalesced path (host-checked)
         float4 rv[8];
 #pragma unroll 1
-        for (int c0 = half * 32; c0 < BN; c0 += 64) {
+        for (int c0 = 0; c0 < BN; c0 += 32) {
           const int n0 = nt * BN + c0;
           const bool vpart = d.out_mode == ALDM_OUT_QKV && n0 >= d.n_split;
           const bool pre = d.res != nullptr && !vpart;
@@ -803,8 +834,9 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
           if (d.bias) add_vec32(v, d.bias + n0);
           if (d.rowvec) add_vec32(v, d.rowvec + (long long)r.b * d.ld_rowvec + n0);
           if (!vpart && pair_qk) {
-            // Q | K planes (one fp16 plane, 64 bytes per row and chunk): full-line stores by the warp pair (emit_pair_hi)
-            emit_pair_hi(d, cr, nt * BN + (c0 & ~63), pair_tiles + ((pair_cnt++ & 1u) ? 4 * (32 * 33 * 4) : 0), lane, half, pair_bar, v);
+            // Q | K planes (one fp16 plane, 64 bytes per row and chunk): full-line stores per 64-column group
+            line_put_hi(stg8, lane, (c0 >> 5) & 1, v);
+            if (c0 & 32) line_store_hi(d, cr, nt * BN + (c0 & ~63), stg8, lane);
           } else if (!vpart) {
             epi_finish_coalesced(d, cr, n0, v, d.N, stg, lane, rv, pre);
           } else if (r.valid) {
@@ -827,7 +859,7 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
       } else {
         // generic: any activation / output mode, row-owner stores
 #pragma unroll 1
-        for (int c0 = half * 32; c0 < BN; c0 += 64) {
+        for (int c0 = 0; c0 < BN; c0 += 32) {
           if (d.act == ALDM_ACT_GEGLU) {
             if (c0 >= BN / 2) break;
             uint32_t vr[32], gr[32];
@@ -843,6 +875,10 @@ __global__ void __launch_bounds__(416, 1) gemm_tc3_kernel(const __grid_constant_
           }
         }
       }
+      if (ew == 0 && lane == 0) ALDM_TL(3, tl, 1);
+      // every lane's reads of the accumulator tile are done: the consumers may overwrite it
+      __syncwarp();
+      if (lane == 0) mbar_arrive(acc_empty);
     }
   }
 }
@@ -1047,7 +1083,7 @@ static int launch_tc3_ap(const aldm_gemm_desc& d, int M, const GemmVariant& v, c
   fd.plain = d.ntaps == 1 && d.dy[0] == 0 && d.dx[0] == 0 && d.sy == 1 && d.sx == 1 && d.up == 0 && d.bmod <= 0 &&
              d.OH == d.H && d.OW == d.W;
   fd.store = v.store;
-  ALDM_CHECK_CUDA(launch_pdl(gemm_tc3_kernel<BN, EPI, AP>, dim3(grid), dim3(416), C::SMEM_BYTES, st, d, tiles_m, tiles_n, fd));
+  ALDM_CHECK_CUDA(launch_pdl(gemm_tc3_kernel<BN, EPI, AP>, dim3(grid), dim3(512), C::SMEM_BYTES, st, d, tiles_m, tiles_n, fd));
   ALDM_CHECK_CUDA(cudaGetLastError());
   if (d.splitk > 1) {
     const int Mpad = tiles_m * C::BM, Npad = tiles_n * BN;
@@ -1096,6 +1132,7 @@ static int gemm_check(const aldm_gemm_desc& d) {
   ALDM_REQUIRE(d.a_hi, ALDM_E_ARG, "gemm: null A plane");      // a_lo == NULL: single-plane activations
   ALDM_REQUIRE(aligned16(d.a_hi) && aligned16(d.a_lo), ALDM_E_ALIGN, "gemm: A planes not 16B aligned");
   ALDM_REQUIRE(d.up == 0 || d.up == 1, ALDM_E_ARG, "gemm: up=%d", d.up);
+  ALDM_REQUIRE(d.up == 0 || (d.H < 65536 && d.W < 65536), ALDM_E_SHAPE, "gemm: upsampled input %dx%d too large", d.H, d.W);
   ALDM_REQUIRE(d.splitk >= 1 && d.splitk <= d.Kpad / 64, ALDM_E_ARG, "gemm: splitk=%d", d.splitk);
   ALDM_REQUIRE(d.splitk == 1 || d.ws, ALDM_E_ARG, "gemm: split-K needs a workspace");
   if (d.act == ALDM_ACT_GEGLU) {

@@ -126,8 +126,9 @@ int aldm_gemm(const aldm_gemm_desc* d, void* stream);
  * Epilogue bodies: FAST (bias / row vector / residual, fp32 / planes / dual / QKV outputs), GEGLU, GENERIC (everything
  * else, and every split-K GEMM), F32N / PLN (compact bodies: fp32 / plane output with bias and residual only).
  * Reductions: REDUCE4 (coalesced, no activation / alpha / accumulate; fp32, planes or dual out), GENERIC (any epilogue).
- * Store modes: ROW (per-warp rows), COMPACT (swizzled staging tile of the compact bodies), PAIR_* (two warps assemble
- * full 128-byte fp16 lines: single-plane PLN output, GEGLU planes output, Q|K columns of a QKV output).
+ * Store modes: ROW (per-warp rows), COMPACT (swizzled staging tile of the compact bodies), PAIR_* (a warp assembles the
+ * two 32-column chunks of a 64-column group into full 128-byte fp16 lines: single-plane PLN output, GEGLU planes output,
+ * Q|K columns of a QKV output).
  * Returns ALDM_E_UNSUPPORTED for the SIMT checker (impl = ALDM_GEMM_SIMT) and the aldm_gemm error for a bad descriptor. */
 enum { ALDM_EPI_FAST = 0, ALDM_EPI_GEGLU = 1, ALDM_EPI_GENERIC = 2, ALDM_EPI_F32N = 3, ALDM_EPI_PLN = 4 };
 enum { ALDM_RED_NONE = 0, ALDM_RED_REDUCE4 = 1, ALDM_RED_GENERIC = 2 };
