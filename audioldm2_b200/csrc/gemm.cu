@@ -635,6 +635,13 @@ __global__ void __launch_bounds__(512, 1) gemm_tc3_kernel(const __grid_constant_
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       for (int it = 0; it < nkb; ++it, ++cnt) {
         const int s = cnt % C::STAGES;
+        // Release the previous stage as soon as its MMAs have completed, BEFORE waiting for this one.  Released after
+        // this stage's wait, a slot whose MMAs are long done stays held while the consumers wait for data, so one load
+        // fewer is in flight: with two stages (BN = 128, two A planes: the convolutions) only one.
+        if (it > 0) {
+          wgmma_wait<0>();
+          if (lane == 0) mbar_arrive(empty_bar((cnt - 1) % C::STAGES));
+        }
         mbar_wait(full_bar(s), (cnt / C::STAGES) & 1);
         if (tid == 0) ALDM_TL(2, cnt, 0);
         fence_proxy_async();          // cp.async-written A tiles -> visible to the tensor core (async proxy)
@@ -654,8 +661,6 @@ __global__ void __launch_bounds__(512, 1) gemm_tc3_kernel(const __grid_constant_
           }
         }
         wgmma_commit();
-        wgmma_wait<1>();              // the previous stage's MMAs have completed: release it
-        if (it > 0 && lane == 0) mbar_arrive(empty_bar((cnt - 1) % C::STAGES));
         if (tid == 0) ALDM_TL(2, cnt, 1);
       }
       wgmma_wait<0>();

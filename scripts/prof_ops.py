@@ -95,7 +95,16 @@ def build(name, impl):
         ios["src"] = ("f32", src.ref, (rows, Cc)); ins["src"] = torch.randn(rows, Cc, generator=g)
         flops = 0.0
     pl = P.finish(ios)
-    return pl, ins, first, flops
+    return pl, ins, first, flops, sum(operand_bytes(o) for o in pl.ops[first:] if o["kind"] == "gemm")
+
+
+def operand_bytes(o) -> int:
+    """Bytes one GEMM launch moves from L2 into shared memory: every 128-row tile gathers its A rows (K fp16 values per
+    plane) and receives its own copy of the [hi | lo] weight image of its N tile (Kpad x bn x 2 planes)."""
+    M = o["B"] * o["OH"] * o["OW"]
+    tiles_m, tiles_n = math.ceil(M / 128), math.ceil(o["N"] / o["bn"])
+    ap = 2 if o["a_lo"] is not None else 1
+    return tiles_m * tiles_n * (128 * o["K"] * 2 * ap + o["bn"] * o["Kpad"] * 4)
 
 
 def main():
@@ -109,11 +118,11 @@ def main():
     global TOK
     TOK = a.planes
     dev = torch.device("cuda:0")
-    print(f"{'case':28s} {'us/launch':>10s} {'TFLOP/s':>9s}")
+    print(f"{'case':28s} {'us/launch':>10s} {'TFLOP/s':>9s} {'A+B MB':>8s} {'A+B TB/s':>9s}")
     for name in CASES:
         if a.only and name not in a.only.split(","):
             continue
-        pl, ins, first, flops = build(name, a.impl)
+        pl, ins, first, flops, nbytes = build(name, a.impl)
         if a.dbg:
             for o in pl.ops:
                 if o["kind"] == "gemm":
@@ -130,7 +139,8 @@ def main():
             prog.run("op")
         e1.record(); torch.cuda.synchronize()
         us = e0.elapsed_time(e1) * 1e3 / a.reps
-        print(f"{name:28s} {us:10.1f} {flops / (us * 1e-6) / 1e12 if flops else 0:9.1f}", flush=True)
+        print(f"{name:28s} {us:10.1f} {flops / (us * 1e-6) / 1e12 if flops else 0:9.1f} {nbytes / 1e6:8.1f} "
+              f"{nbytes / (us * 1e-6) / 1e12:9.2f}", flush=True)
         if a.dbg & 128:
             import ctypes as C
             buf = (C.c_longlong * (4 * 256 * 2))()
