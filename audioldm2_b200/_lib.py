@@ -35,6 +35,7 @@ OUT_F32, OUT_PLANES, OUT_NCHW, OUT_QKV = 0, 1, 2, 3
 EPI_FAST, EPI_GEGLU, EPI_GENERIC, EPI_F32N, EPI_PLN = 0, 1, 2, 3, 4              # aldm_gemm_variant out[1]
 RED_NONE, RED_REDUCE4, RED_GENERIC = 0, 1, 2                                     # out[3]
 STORE_ROW, STORE_COMPACT, STORE_PAIR_PLN, STORE_PAIR_GEGLU, STORE_PAIR_QK = 0, 1, 2, 3, 4   # out[4]
+AMODE_GATHER, AMODE_HALO = 0, 1                                                   # aldm_gemm_a_mode
 PREP_COPY, PREP_SILU, PREP_LRELU, PREP_GN, PREP_GN_SILU, PREP_LN = 0, 1, 2, 3, 4, 5
 OP_GEMM, OP_PREP, OP_ATTN, OP_SOFTMAX, OP_TEMB, OP_TRANSPOSE, OP_PACKB, OP_COPY = 1, 2, 3, 4, 5, 6, 7, 8
 OP_SEQ_ASSEMBLE, OP_KV_ATTN, OP_SEQ_FEEDBACK = 9, 10, 11
@@ -199,6 +200,7 @@ def lib() -> C.CDLL:
     sig = {
         "aldm_gemm": (i32, [C.POINTER(GemmDesc), vp]),
         "aldm_gemm_variant": (i32, [C.POINTER(GemmDesc), C.POINTER(i32)]),
+        "aldm_gemm_a_mode": (i32, [C.POINTER(GemmDesc), C.POINTER(i32)]),
         "aldm_prep": (i32, [C.POINTER(PrepDesc), vp]),
         "aldm_pack_b": (i32, [vp, i32, i32, i32, i32, i32, vp, vp, vp]),
         "aldm_attention": (i32, [C.POINTER(AttnDesc), vp]),
@@ -253,7 +255,7 @@ def lib() -> C.CDLL:
     return L
 
 
-EXPORTED = ["aldm_gemm", "aldm_gemm_variant", "aldm_prep", "aldm_pack_b", "aldm_attention", "aldm_softmax_rows",
+EXPORTED = ["aldm_gemm", "aldm_gemm_variant", "aldm_gemm_a_mode", "aldm_prep", "aldm_pack_b", "aldm_attention", "aldm_softmax_rows",
             "aldm_kv_attention", "aldm_seq_assemble", "aldm_seq_feedback",
             "aldm_timestep_embedding", "aldm_ddim_step", "aldm_masked_blend", "aldm_transpose_chw",
             "aldm_posterior_sample", "aldm_stft_mel", "aldm_program_create", "aldm_program_run",
@@ -271,6 +273,13 @@ def gemm_variant(d: GemmDesc) -> tuple:
     out = (C.c_int32 * 5)()
     check(lib().aldm_gemm_variant(C.byref(d), out), "gemm_variant")
     return tuple(out)
+
+
+def gemm_a_mode(d: GemmDesc) -> int:
+    """aldm_gemm_a_mode: AMODE_GATHER or AMODE_HALO, how the kernel aldm_gemm runs for `d` loads A (no GPU needed)."""
+    out = C.c_int32()
+    check(lib().aldm_gemm_a_mode(C.byref(d), C.byref(out)), "gemm_a_mode")
+    return out.value
 
 
 def check(rc: int, what: str = ""):

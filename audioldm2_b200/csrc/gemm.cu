@@ -20,6 +20,11 @@
 //               pre-swizzled weight tile image (hi|lo) per stage.
 //   warps 12-15 epilogue warpgroup: warp w finishes rows [32 w, 32 w + 32) of the tile, all BN columns, while the
 //               consumers already run the next tile's MMAs.
+// Halo A path (HALO = 1, aldm_gemm_a_mode): for a 3x3, stride-1 convolution (nearest x2 upsample folded in or not) an M
+// tile is an 8 x 16 or 16 x 8 pixel block.
+// Warps 8-10 copy its 180-pixel input halo once per 64-channel block into a slab (cp.async, zero fill = the padding), one
+// lane of warp 11 streams one tap's weight tile per stage, and the consumers issue the nine taps from the slab through
+// shifted descriptors: the A bytes per tile drop from 9 x 128 to 180 pixel rows.  The K loop runs (channel block, tap).
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -314,32 +319,49 @@ __device__ __forceinline__ void line_store_hi(const aldm_gemm_desc& d, const CR&
 // ------------------------------------------------------------------------------------------
 // tensor-core kernel
 // ------------------------------------------------------------------------------------------
-template <int BN, int AP>
+// Shared memory, in order: [halo slab (HALO only)] [STAGES stages] [fp32 accumulator] [barriers] [epilogue staging].
+// Gather (HALO = 0): a stage is [a_hi | a_lo (AP == 2)] [b_hi | b_lo].  BN = 128: 2 stages (AP 2) / 3 (AP 1); BN = 64:
+// 3 / 4; BN = 32: 4.
+// Halo (HALO = 1, BN = 64 only): the A operand of one 64-channel block is a slab of the tile's (th + 2) x (tw + 2) = 180
+// input pixels, 128 bytes each, per plane, rounded up to the 1024-byte swizzle atom: 23,552 B.  Two slabs, so that the
+// next channel block loads while the MMAs run on this one; a stage holds one tap's weight tile [b_hi | b_lo] (16 KB).
+// Budget (bytes): 232,448 - 32,768 accumulator - 16,896 staging - 1,280 alignment and barriers = 181,504 =
+// 2 x AP x 23,552 slabs + 4 x 16,384 stages + 21,760 (AP 2) / 68,864 (AP 1) spare.  At BN = 128 the 64 KB accumulator
+// leaves room for one slab only (148,736 = 2 x 23,552 + 3 x 32,768 + 3,328): every channel block then waits for its
+// slab with the tensor cores idle, and that variant was slower (DESIGN.md section 5b).
+template <int BN, int AP, int HALO = 0>
 struct Tc3Cfg {
   static constexpr int BM = 128;
   static constexpr int BK = 64;                       // fp16 elements = 128 bytes per row
   static constexpr int A_BYTES = BM * 128;            // one plane
   static constexpr int B_BYTES = BN * 128;            // one plane
-  static constexpr int STAGE_BYTES = AP * A_BYTES + 2 * B_BYTES;      // [a_hi | a_lo (AP == 2)] [b_hi | b_lo]
-  static constexpr int B_OFF = AP * A_BYTES;
+  static constexpr int HALO_PIX = 180;                // (8 + 2) x (16 + 2) or (16 + 2) x (8 + 2)
+  static constexpr int SLAB_PLANE = HALO ? (HALO_PIX * 128 + 1023) / 1024 * 1024 : 0;
+  static constexpr int NSLAB = HALO ? 2 : 0;
+  static constexpr int SLAB_SET = AP * SLAB_PLANE;     // one slab: [a_hi | a_lo (AP == 2)]
+  static constexpr int SLAB_BYTES = NSLAB * SLAB_SET;
+  static constexpr int STAGE_BYTES = (HALO ? 0 : AP * A_BYTES) + 2 * B_BYTES;
+  static constexpr int B_OFF = HALO ? 0 : AP * A_BYTES;
   static constexpr int ACC_BYTES = BM * BN * 4;       // fp32 accumulator tile handed from the warpgroups to the epilogue
   static constexpr int STG_BYTES = 4 * 32 * 33 * 4;   // one 32x33 fp32 transpose tile per epilogue warp
   static constexpr int SMEM_MAX = 227 * 1024;
-  static constexpr int FIT = (SMEM_MAX - 1024 - 256 - STG_BYTES - ACC_BYTES) / STAGE_BYTES;
-  static constexpr int STAGES = FIT > 4 ? 4 : FIT;    // BN=128: 2 stages (AP 2) / 3 (AP 1); BN=64: 3 / 4; BN=32: 4
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + STG_BYTES;
+  static constexpr int FIT = (SMEM_MAX - 1024 - 256 - STG_BYTES - ACC_BYTES - SLAB_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = FIT > 4 ? 4 : FIT;
+  static constexpr int SMEM_BYTES = SLAB_BYTES + STAGES * STAGE_BYTES + ACC_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + STG_BYTES;
   static_assert(STAGES >= 2, "pipeline needs two stages");
   static_assert(SMEM_BYTES <= SMEM_MAX, "shared memory");
+  static_assert(!HALO || BN == 64, "the halo path is built for BN = 64");
 };
 
 // Accumulator tile in shared memory: row-major fp32 [BM][BN], the 16-byte chunk index XOR-swizzled by (row & 7), so that
 // the wgmma fragment stores and the row-per-lane reads of the epilogue (acc_ld32) are both free of bank conflicts.
+// The fragment's rows g and g + 8 land in tile rows row0 + g and row0 + g + hstep (row0 a multiple of 8).
 template <int BN>
-__device__ __forceinline__ void acc_st_frag(float* accb, int row0, int lane, const float* d) {
+__device__ __forceinline__ void acc_st_frag(float* accb, int row0, int hstep, int lane, const float* d) {
   const int g = lane >> 2, t = lane & 3;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int row = row0 + g + 8 * h;
+    const int row = row0 + g + hstep * h;
     float* rp = accb + row * BN + 2 * (t & 1);
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j)
@@ -363,6 +385,11 @@ __device__ __forceinline__ void acc_ld32(const float* accb, int row, int c0, uin
 // least that holds the producers' per-row state without spilling; no instance spills at this split (ptxas -v).
 constexpr int kProdRegs = 80, kConsRegs = 136, kEpiRegs = 160;
 static_assert(kProdRegs + 2 * kConsRegs + kEpiRegs == 4 * 128, "register split must use exactly the launch allocation");
+// wgmma_desc_sw128 with a stride byte offset of `sbo` bytes between 8-row groups (the halo slab's row pitch).
+__device__ __forceinline__ uint64_t wgmma_desc_sw128_sbo(uint32_t smem_addr, uint32_t sbo) {
+  return static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (static_cast<uint64_t>((sbo >> 4) & 0x3FFFu) << 32) |
+         (1ull << 62);
+}
 template <int R>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R>
@@ -423,22 +450,32 @@ struct Tc3Divs {
   FastDiv ow, oh, cp, tn, bmod;
   int plain;      // 1x1 tap, unit stride, no upsample / batch-modulo: input row == output row (linear layers)
   int store;      // ALDM_STORE_*: decided once on the host (gemm_select), so aldm_gemm_variant reports what runs
+  // halo path: an M tile is a th x tw pixel block of one image (tw = 16, th = 8 or tw = 8, th = 16); tiles are numbered
+  // image, then block row, then block column
+  FastDiv tpi, tx;    // tiles per image, tiles per block row
+  int tw_sh;          // log2(tw)
 };
 
 // AP = number of A planes (2: hi + lo, three MMAs per K step; 1: hi only, two MMAs and half the A bytes).
-template <int BN, int EPI, int AP>
+// HALO = 1 (BN = 64; aldm_gemm_a_mode): the A operand of each 64-channel block is one halo slab per plane and the
+// consumers issue the nine taps of a 3x3 convolution from it (see the halo branches below).
+template <int BN, int EPI, int AP, int HALO>
 __global__ void __launch_bounds__(512, 1) gemm_tc3_kernel(const __grid_constant__ aldm_gemm_desc d, int tiles_m, int tiles_n,
                                                            const __grid_constant__ Tc3Divs fd) {
-  using C = Tc3Cfg<BN, AP>;
+  using C = Tc3Cfg<BN, AP, HALO>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
-  const uint32_t acc_base = base + C::STAGES * C::STAGE_BYTES;
+  const uint32_t slab = base;                                  // HALO: C::NSLAB slabs of C::SLAB_SET bytes
+  auto stage_base = [&](int s) { return base + C::SLAB_BYTES + s * C::STAGE_BYTES; };
+  const uint32_t acc_base = base + C::SLAB_BYTES + C::STAGES * C::STAGE_BYTES;
   const uint32_t bar_base = acc_base + C::ACC_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
   const uint32_t acc_full = bar_base + 8u * (2 * C::STAGES);
   const uint32_t acc_empty = acc_full + 8u;
+  auto slab_full = [&](int i) { return acc_empty + 8u + 8u * i; };                 // HALO only
+  auto slab_empty = [&](int i) { return acc_empty + 8u + 8u * (C::NSLAB + i); };
   float* accb = reinterpret_cast<float*>(smem_raw + (acc_base - raw));
 
   const int tid = threadIdx.x;
@@ -451,11 +488,16 @@ __global__ void __launch_bounds__(512, 1) gemm_tc3_kernel(const __grid_constant_
 
   if (tid == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(full_bar(s), 128 + 1);   // 128 cp.async producers (completion-triggered arrivals) + B expect_tx
+      // gather: 128 cp.async producers (completion-triggered arrivals) + B expect_tx; halo: the B expect_tx alone
+      mbar_init(full_bar(s), HALO ? 1 : 128 + 1);
       mbar_init(empty_bar(s), 8);        // one arrival per consumer warp once its MMAs on the stage have completed
     }
     mbar_init(acc_full, 8);              // one arrival per consumer warp: its rows of the accumulator are in shared memory
     mbar_init(acc_empty, 4);             // one arrival per epilogue warp: done reading the accumulator tile
+    for (int i = 0; i < C::NSLAB; ++i) {
+      mbar_init(slab_full(i), 96);       // the 96 halo producers' cp.async completions
+      mbar_init(slab_empty(i), 8);       // one arrival per consumer warp once its MMAs on the slab have completed
+    }
     fence_barrier_init();
   }
   __syncthreads();
@@ -478,6 +520,101 @@ __global__ void __launch_bounds__(512, 1) gemm_tc3_kernel(const __grid_constant_
   if (warp >= 8 && warp < 12) {
     // ===================== producers: A gather + weight TMA =====================
     setmaxnreg_dec<kProdRegs>();
+    if constexpr (HALO) {
+      // Halo: warps 8-10 load one slab per 64-channel block, one elected lane of warp 11 streams the weight tiles.  The K
+      // loop runs channel block cb outer, tap inner; the weight tile of (tap, cb) is the packed k-block tap * Cp / 64 + cb.
+      // The weights may be packed in d.bn = 128-row tiles: N tile nt is then rows [64 (nt % 2), + 64) of packed tile nt / 2,
+      // one 8 KB run in each plane (a packed plane is 128-byte rows in N order, swizzled by row & 7).
+      const int ncb = d.Cp >> 6;
+      const int tw = 1 << fd.tw_sh, th = C::BM >> fd.tw_sh, hw = tw + 2;
+      if (warp == 11) {
+        if (!(d.impl & ALDM_GEMM_STATIC_B)) pdl_wait();       // the weights are the only global memory this lane reads
+        if (elect_one()) {
+          uint32_t cnt = 0;
+          for (int id = blockIdx.x; id < total; id += gridDim.x) {
+            int mt, nt, z, kb0, nkb;
+            tile_coords(id, mt, nt, z, kb0, nkb);
+            const int per = d.bn / BN;
+            const long long wtile = 2ll * d.bn * 128;          // bytes of one packed (n tile, k-block) image
+            const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(d.w_packed) + (long long)(nt / per) * nkb_total * wtile +
+                                  (nt % per) * C::B_BYTES;
+            for (int cb = 0; cb < ncb; ++cb)
+              for (int tap = 0; tap < 9; ++tap, ++cnt) {
+                const int s = cnt % C::STAGES;
+                mbar_wait(empty_bar(s), ((cnt / C::STAGES) & 1) ^ 1);
+                if (dbg & 2) { mbar_arrive(full_bar(s)); continue; }
+                const uint8_t* src = wsrc + (long long)(tap * ncb + cb) * wtile;
+                mbar_arrive_expect_tx(full_bar(s), 2 * C::B_BYTES);
+                bulk_g2s(stage_base(s), src, C::B_BYTES, full_bar(s));
+                bulk_g2s(stage_base(s) + C::B_BYTES, src + wtile / 2, C::B_BYTES, full_bar(s));
+              }
+          }
+        }
+        return;
+      }
+      // 180 halo pixels x 8 chunks of 16 bytes = 96 threads x 15 copies per plane: thread pt copies chunk j = pt & 7 of halo
+      // pixels hr0 + 12 i (i < 15), into the slab row hr with the 128-byte swizzle (chunk j ^ (hr & 7)), the layout the
+      // wgmma descriptors read.  12 i changes hr & 7 by 4 i: even and odd i have one destination base each.
+      const int pt = tid - 256;
+      const int j = pt & 7, hr0 = pt >> 3;
+      // up = 1 (nearest x2 upsample folded in): halo pixel (hy, hx) at full resolution is source pixel
+      // ((y0 - 1 + hy) >> 1, (x0 - 1 + hx) >> 1) = (y0 / 2 + ((hy - 1) >> 1), x0 / 2 + ((hx - 1) >> 1)), y0 and x0 being even
+      const int Ws = d.W >> d.up;
+      int relc[15];                              // element offset of each pixel from source pixel (y0 >> up, x0 >> up)
+      uint32_t e_top = 0, e_bot = 0, e_lft = 0, e_rgt = 0;     // bit i: pixel i is on that edge of the halo
+#pragma unroll
+      for (int i = 0; i < 15; ++i) {
+        const int hr = hr0 + 12 * i, hy = hr / hw, hx = hr - hy * hw;
+        relc[i] = (((hy - 1) >> d.up) * Ws + ((hx - 1) >> d.up)) * d.Cp;
+        e_top |= (uint32_t)(hy == 0) << i;
+        e_bot |= (uint32_t)(hy == th + 1) << i;
+        e_lft |= (uint32_t)(hx == 0) << i;
+        e_rgt |= (uint32_t)(hx == tw + 1) << i;
+      }
+      const uint32_t d_even = slab + hr0 * 128 + ((j ^ (hr0 & 7)) << 4);
+      const uint32_t d_odd = slab + hr0 * 128 + ((j ^ ((hr0 + 4) & 7)) << 4);
+      const aldm_plane_t* ahi = reinterpret_cast<const aldm_plane_t*>(d.a_hi);
+      const aldm_plane_t* alo = reinterpret_cast<const aldm_plane_t*>(d.a_lo);
+      uint32_t cnt = 0;
+      pdl_wait();
+      for (int id = blockIdx.x; id < total; id += gridDim.x) {
+        int mt, nt, z, kb0, nkb, b, t, ty, tx;
+        tile_coords(id, mt, nt, z, kb0, nkb);
+        fd.tpi.divmod(mt, b, t);
+        fd.tx.divmod(t, ty, tx);
+        const int y0 = ty * th, x0 = tx * tw;
+        int bs = b;
+        if (d.bmod > 0) { int q; fd.bmod.divmod(b, q, bs); }
+        // the border pixels outside the image are the convolution's zero padding (cp.async zero fill)
+        uint32_t valid = 0x7fffu;
+        if (y0 == 0) valid &= ~e_top;
+        if (y0 + th == d.H) valid &= ~e_bot;
+        if (x0 == 0) valid &= ~e_lft;
+        if (x0 + tw == d.W) valid &= ~e_rgt;
+        const long long pix0 = ((long long)(bs * (d.H >> d.up) + (y0 >> d.up)) * Ws + (x0 >> d.up)) * d.Cp + j * 8;
+        for (int cb = 0; cb < ncb; ++cb, ++cnt) {
+          const int sl = cnt % C::NSLAB;
+          mbar_wait(slab_empty(sl), ((cnt / C::NSLAB) & 1) ^ 1);
+          const uint32_t de = d_even + sl * C::SLAB_SET, dod = d_odd + sl * C::SLAB_SET;
+          if (!(dbg & 1)) {
+            const aldm_plane_t* ab = ahi + pix0 + cb * 64;
+            const aldm_plane_t* abl = alo + pix0 + cb * 64;
+#define ALDM_HALO_PIX(i)                                                                                   \
+            {                                                                                                \
+              const uint32_t nb = ((valid >> (i)) & 1u) << 4;                                                \
+              cp_async_16_off<(i) * 1536>((i) & 1 ? dod : de, ab + relc[i], nb);                             \
+              if (AP == 2) cp_async_16_off<(i) * 1536 + C::SLAB_PLANE>((i) & 1 ? dod : de, abl + relc[i], nb); \
+            }
+            ALDM_HALO_PIX(0) ALDM_HALO_PIX(1) ALDM_HALO_PIX(2) ALDM_HALO_PIX(3) ALDM_HALO_PIX(4) ALDM_HALO_PIX(5)
+            ALDM_HALO_PIX(6) ALDM_HALO_PIX(7) ALDM_HALO_PIX(8) ALDM_HALO_PIX(9) ALDM_HALO_PIX(10) ALDM_HALO_PIX(11)
+            ALDM_HALO_PIX(12) ALDM_HALO_PIX(13) ALDM_HALO_PIX(14)
+#undef ALDM_HALO_PIX
+          }
+          cp_async_mbar_arrive_noinc(slab_full(sl));
+        }
+      }
+      return;
+    }
     const int ptid = tid - 256;
     const int j = ptid & 7;                 // 16-byte chunk (8 channels) inside the 64-wide K block
     const int rbase = ptid >> 3;            // rows rbase + 16*i
@@ -625,6 +762,69 @@ __global__ void __launch_bounds__(512, 1) gemm_tc3_kernel(const __grid_constant_
     setmaxnreg_inc<kConsRegs>();
     pdl_wait();
     const int wg = warp >> 2;
+    if constexpr (HALO) {
+      // Warpgroup wg computes 64 pixels of the tile as eight groups of 8 consecutive pixels of one row: tw = 16, columns
+      // [8 wg, 8 wg + 8) of the 8 rows; tw = 8, rows [8 wg, 8 wg + 8).  In the slab the groups start one halo row (hw x 128
+      // bytes, the descriptor's stride byte offset) apart, and tap (dy, dx) moves the start by dy hw + dx whole 128-byte
+      // rows.  The hardware applies the 128-byte swizzle to the address it computes, and the slab is written swizzled by
+      // its absolute row, so a window that starts at any row reads the slab as written.
+      const int ncb = d.Cp >> 6;
+      const int tw = 1 << fd.tw_sh, hw = tw + 2;
+      const int row_c = (tw == 8 ? 8 * wg + 1 : 1) * hw + (tw == 16 ? 8 * wg : 0) + 1;     // tap (0, 0)
+      const uint32_t sbo = (uint32_t)hw * 128u;
+      uint32_t cnt = 0, scnt = 0, tl = 0;
+      float acc[BN / 2];
+      for (int id = blockIdx.x; id < total; id += gridDim.x, ++tl) {
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        for (int cb = 0; cb < ncb; ++cb, ++scnt) {
+          const int sl = scnt % C::NSLAB;
+          if (cb > 0) {     // the previous block's last weight stage and its slab, once their MMAs have completed
+            wgmma_wait<0>();
+            if (lane == 0) { mbar_arrive(empty_bar((cnt - 1) % C::STAGES)); mbar_arrive(slab_empty((scnt - 1) % C::NSLAB)); }
+          }
+          mbar_wait(slab_full(sl), (scnt / C::NSLAB) & 1);
+          fence_proxy_async();        // cp.async-written slab -> visible to the tensor core (async proxy)
+#pragma unroll 1
+          for (int tap = 0; tap < 9; ++tap, ++cnt) {
+            const int s = cnt % C::STAGES;
+            if (tap > 0) {
+              wgmma_wait<0>();
+              if (lane == 0) mbar_arrive(empty_bar((cnt - 1) % C::STAGES));
+            }
+            mbar_wait(full_bar(s), (cnt / C::STAGES) & 1);
+            const uint32_t sa = slab + sl * C::SLAB_SET + (uint32_t)(row_c + d.dy[tap] * hw + d.dx[tap]) * 128u;
+            const uint64_t da_hi = wgmma_desc_sw128_sbo(sa, sbo);
+            const uint64_t da_lo = wgmma_desc_sw128_sbo(sa + C::SLAB_PLANE, sbo);      // only used when AP == 2
+            const uint64_t db_hi = wgmma_desc_sw128(stage_base(s));
+            const uint64_t db_lo = wgmma_desc_sw128(stage_base(s) + C::B_BYTES);
+            wgmma_fence();
+            if (!(dbg & 4)) {
+#pragma unroll
+              for (int ks = 0; ks < 4; ++ks) {
+                const uint64_t o = (uint64_t)(ks * 2);
+                wgmma_ss<BN>(acc, da_hi + o, db_lo + o, 1);
+                if (AP == 2) wgmma_ss<BN>(acc, da_lo + o, db_hi + o, 1);
+                wgmma_ss<BN>(acc, da_hi + o, db_hi + o, 1);
+              }
+            }
+            wgmma_commit();
+          }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs<BN / 2>(acc);
+        if (lane == 0) { mbar_arrive(empty_bar((cnt - 1) % C::STAGES)); mbar_arrive(slab_empty((scnt - 1) % C::NSLAB)); }
+        if (tid == 0 && id + (int)gridDim.x >= total) pdl_launch();
+        mbar_wait(acc_empty, (tl & 1) ^ 1);
+        // tile row of pixel (y, x) = y tw + x.  tw = 16: this warp's fragment rows g and g + 8 are pixel groups
+        // 2 (warp & 3) and 2 (warp & 3) + 1, i.e. tile rows 32 (warp & 3) + 8 wg + g and 16 further; tw = 8: the gather's order.
+        if (tw == 16) acc_st_frag<BN>(accb, 32 * (warp & 3) + 8 * wg, 16, lane, acc);
+        else acc_st_frag<BN>(accb, wg * 64 + (warp & 3) * 16, 8, lane, acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(acc_full);
+      }
+      return;
+    }
     uint32_t cnt = 0, tl = 0;
     float acc[BN / 2];
     for (int id = blockIdx.x; id < total; id += gridDim.x, ++tl) {
@@ -670,7 +870,7 @@ __global__ void __launch_bounds__(512, 1) gemm_tc3_kernel(const __grid_constant_
       if (tid == 0 && id + (int)gridDim.x >= total) pdl_launch();
       // hand the accumulator over once the epilogue is done reading the previous tile's
       mbar_wait(acc_empty, (tl & 1) ^ 1);
-      acc_st_frag<BN>(accb, wg * 64 + (warp & 3) * 16, lane, acc);
+      acc_st_frag<BN>(accb, wg * 64 + (warp & 3) * 16, 8, lane, acc);
       __syncwarp();
       if (lane == 0) mbar_arrive(acc_full);
     }
@@ -697,7 +897,16 @@ __global__ void __launch_bounds__(512, 1) gemm_tc3_kernel(const __grid_constant_
       tile_coords(id, mt, nt, z, kb0, nkb);
       const int m = mt * C::BM + trow_in_tile;
       RowInfo r;
-      {
+      if (HALO) {        // tile mt = (image, block row, block column), tile row = y tw + x; every row is inside the image
+        int t, ty, tx;
+        fd.tpi.divmod(mt, r.b, t);
+        fd.tx.divmod(t, ty, tx);
+        r.oh = ty * (C::BM >> fd.tw_sh) + (trow_in_tile >> fd.tw_sh);
+        r.ow = (tx << fd.tw_sh) + (trow_in_tile & ((1 << fd.tw_sh) - 1));
+        r.m = (r.b * d.OH + r.oh) * d.OW + r.ow;
+        r.valid = true;
+        r.orow = ((long long)r.b * d.OHF + (long long)r.oh * d.osy + d.ooy) * d.OWF + r.ow;
+      } else {
         r.m = m; r.valid = m < M;
         const int mm = r.valid ? m : 0;
         int t;
@@ -1031,12 +1240,25 @@ __global__ void gemm_simt_kernel(const __grid_constant__ aldm_gemm_desc d, int N
 // The kernel variant a descriptor runs: template parameters (BN, EPI, AP), split-K reduction kernel and store mode.  One
 // function decides it for the launch and for aldm_gemm_variant, so what the query reports is what runs.
 struct GemmVariant {
-  int bn, epi, ap, red, store;
+  int bn, epi, ap, red, store, amode;
 };
 
+// The halo A path (aldm_gemm_a_mode): a 3x3, stride-1 convolution whose pixels tile into 8 x 16 or 16 x 8 blocks.
+static bool halo_ok(const aldm_gemm_desc& d) {
+  static const bool on = [] { const char* e = getenv("ALDM_CONV_HALO"); return !(e && e[0] == '0'); }();   // A/B switch
+  if (!on || (d.bn != 64 && d.bn != 128) || d.act == ALDM_ACT_GEGLU || d.splitk != 1 || d.ntaps != 9 || d.sy != 1 ||
+      d.sx != 1 || d.Cp % 64 != 0 || d.OH != d.H || d.OW != d.W)
+    return false;
+  for (int t = 0; t < d.ntaps; ++t)
+    if (d.dy[t] < -1 || d.dy[t] > 1 || d.dx[t] < -1 || d.dx[t] > 1) return false;
+  return (d.W % 16 == 0 && d.H % 8 == 0) || (d.W == 8 && d.H % 16 == 0);
+}
+
 static GemmVariant gemm_select(const aldm_gemm_desc& d) {
-  GemmVariant v{d.bn, EPI_GENERIC, d.a_lo ? 2 : 1, ALDM_RED_NONE, ALDM_STORE_ROW};
-  const int BN = d.bn;
+  const bool halo = halo_ok(d);
+  // the halo kernel runs 64-wide N tiles (two of them per 128-wide packed weight tile)
+  GemmVariant v{halo ? 64 : d.bn, EPI_GENERIC, d.a_lo ? 2 : 1, ALDM_RED_NONE, ALDM_STORE_ROW, halo ? ALDM_AMODE_HALO : ALDM_AMODE_GATHER};
+  const int BN = v.bn;
   // pick the specialised epilogue: the planner's dominant cases take the compact bodies
   const bool geglu = d.act == ALDM_ACT_GEGLU;
   const int n_out = geglu ? d.N / 2 : d.N;
@@ -1071,12 +1293,12 @@ static GemmVariant gemm_select(const aldm_gemm_desc& d) {
   return v;
 }
 
-template <int BN, int EPI, int AP>
-static int launch_tc3_ap(const aldm_gemm_desc& d, int M, const GemmVariant& v, cudaStream_t st) {
-  using C = Tc3Cfg<BN, AP>;
+template <int BN, int EPI, int AP, int HALO>
+static int launch_tc3_mode(const aldm_gemm_desc& d, int M, const GemmVariant& v, cudaStream_t st) {
+  using C = Tc3Cfg<BN, AP, HALO>;
   static bool configured = false;
   if (!configured) {
-    ALDM_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc3_kernel<BN, EPI, AP>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    ALDM_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc3_kernel<BN, EPI, AP, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     configured = true;
   }
   const int tiles_m = cdiv(M, C::BM), tiles_n = cdiv(d.N, BN);
@@ -1088,7 +1310,11 @@ static int launch_tc3_ap(const aldm_gemm_desc& d, int M, const GemmVariant& v, c
   fd.plain = d.ntaps == 1 && d.dy[0] == 0 && d.dx[0] == 0 && d.sy == 1 && d.sx == 1 && d.up == 0 && d.bmod <= 0 &&
              d.OH == d.H && d.OW == d.W;
   fd.store = v.store;
-  ALDM_CHECK_CUDA(launch_pdl(gemm_tc3_kernel<BN, EPI, AP>, dim3(grid), dim3(512), C::SMEM_BYTES, st, d, tiles_m, tiles_n, fd));
+  fd.tw_sh = d.W == 8 ? 3 : 4;
+  const int tw = 1 << fd.tw_sh, th = C::BM / tw;
+  fd.tx = make_fastdiv(HALO ? d.W / tw : 1);
+  fd.tpi = make_fastdiv(HALO ? (d.H / th) * (d.W / tw) : 1);
+  ALDM_CHECK_CUDA(launch_pdl(gemm_tc3_kernel<BN, EPI, AP, HALO>, dim3(grid), dim3(512), C::SMEM_BYTES, st, d, tiles_m, tiles_n, fd));
   ALDM_CHECK_CUDA(cudaGetLastError());
   if (d.splitk > 1) {
     const int Mpad = tiles_m * C::BM, Npad = tiles_n * BN;
@@ -1104,6 +1330,13 @@ static int launch_tc3_ap(const aldm_gemm_desc& d, int M, const GemmVariant& v, c
     ALDM_CHECK_CUDA(cudaGetLastError());
   }
   return ALDM_OK;
+}
+
+template <int BN, int EPI, int AP>
+static int launch_tc3_ap(const aldm_gemm_desc& d, int M, const GemmVariant& v, cudaStream_t st) {
+  if constexpr (BN == 64)
+    if (v.amode == ALDM_AMODE_HALO) return launch_tc3_mode<BN, EPI, AP, 1>(d, M, v, st);
+  return launch_tc3_mode<BN, EPI, AP, 0>(d, M, v, st);
 }
 
 template <int BN, int EPI>
@@ -1205,6 +1438,15 @@ extern "C" int aldm_gemm_variant(const aldm_gemm_desc* d, int32_t out[5]) {
   if ((d->impl & 0xff) == ALDM_GEMM_SIMT) { aldm::set_error("aldm_gemm_variant: the SIMT checker has no variants"); return ALDM_E_UNSUPPORTED; }
   const aldm::GemmVariant v = aldm::gemm_select(*d);
   out[0] = v.bn; out[1] = v.epi; out[2] = v.ap; out[3] = v.red; out[4] = v.store;
+  return ALDM_OK;
+}
+
+extern "C" int aldm_gemm_a_mode(const aldm_gemm_desc* d, int32_t* mode) {
+  if (!d || !mode) { aldm::set_error("aldm_gemm_a_mode: null argument"); return ALDM_E_ARG; }
+  const int rc = aldm::gemm_check(*d);
+  if (rc) return rc;
+  if ((d->impl & 0xff) == ALDM_GEMM_SIMT) { aldm::set_error("aldm_gemm_a_mode: the SIMT checker has no variants"); return ALDM_E_UNSUPPORTED; }
+  *mode = aldm::gemm_select(*d).amode;
   return ALDM_OK;
 }
 

@@ -134,6 +134,14 @@ enum { ALDM_EPI_FAST = 0, ALDM_EPI_GEGLU = 1, ALDM_EPI_GENERIC = 2, ALDM_EPI_F32
 enum { ALDM_RED_NONE = 0, ALDM_RED_REDUCE4 = 1, ALDM_RED_GENERIC = 2 };
 enum { ALDM_STORE_ROW = 0, ALDM_STORE_COMPACT = 1, ALDM_STORE_PAIR_PLN = 2, ALDM_STORE_PAIR_GEGLU = 3, ALDM_STORE_PAIR_QK = 4 };
 int aldm_gemm_variant(const aldm_gemm_desc* d, int32_t out[5]);
+/* How the tensor-core kernel loads A for `d` (no CUDA calls): GATHER fetches every (tap, pixel) row of the implicit GEMM
+ * separately; HALO loads each 64-channel block of a 3x3, stride-1 convolution's input tile once, with its one-pixel
+ * border, and issues all nine taps from that one copy.  HALO is chosen for bn = 64 or 128 (the kernel then runs 64-wide N
+ * tiles, which aldm_gemm_variant reports), no GEGLU, no split-K, nine taps within one pixel, sy = sx = 1 (up = 0 or 1),
+ * Cp % 64 == 0, and W % 16 == 0 with H % 8 == 0 (8 x 16-pixel tiles) or W == 8 with H % 16 == 0 (16 x 8).
+ * ALDM_CONV_HALO=0 in the environment turns it off. */
+enum { ALDM_AMODE_GATHER = 0, ALDM_AMODE_HALO = 1 };
+int aldm_gemm_a_mode(const aldm_gemm_desc* d, int32_t* mode);
 
 /* ---- operand preparation (normalise / activate / split into bf16 hi+lo planes) ----------- */
 

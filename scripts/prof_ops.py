@@ -30,6 +30,11 @@ CASES = {
     "lin_k640_n5120_geglu": ("gemm", dict(B=1, H=1024, W=1, Cin=640, N=5120, taps=((0, 0),), geglu=True)),
     "conv_l1_128": ("gemm", dict(B=16, H=256, W=16, Cin=128, N=128, taps=plan.TAPS_3x3, res=True)),
     "conv_l2_256": ("gemm", dict(B=16, H=128, W=8, Cin=256, N=256, taps=plan.TAPS_3x3, res=True)),
+    "conv_l1_128_k2304": ("gemm", dict(B=16, H=256, W=16, Cin=256, N=128, taps=plan.TAPS_3x3, res=True)),
+    "conv_l1_128_k3456": ("gemm", dict(B=16, H=256, W=16, Cin=384, N=128, taps=plan.TAPS_3x3, res=True)),
+    "conv_l2_256_k5760": ("gemm", dict(B=16, H=128, W=8, Cin=640, N=256, taps=plan.TAPS_3x3, res=True)),
+    "conv_l2_256_k4608": ("gemm", dict(B=16, H=128, W=8, Cin=512, N=256, taps=plan.TAPS_3x3, res=True)),
+    "conv_up_l1_256": ("gemm", dict(B=16, H=256, W=16, Cin=256, N=256, taps=plan.TAPS_3x3, up=1)),
     "conv_l4_640": ("gemm", dict(B=16, H=32, W=2, Cin=640, N=640, taps=plan.TAPS_3x3, res=True)),
     "attn_1024": ("attn", dict(B=16, heads=8, N=1024)),
     "attn_256": ("attn", dict(B=16, heads=12, N=256)),
@@ -57,7 +62,7 @@ def build(name, impl):
         first = len(P.ops)
         wm = torch.randn(N, len(taps) * Cin, generator=g) / math.sqrt(len(taps) * Cin)
         M = B * H * W
-        kw = dict(B=B, H=H, W=W, taps=taps)
+        kw = dict(B=B, H=H, W=W, taps=taps, up=p.get("up", 0))
         if p.get("geglu"):
             w = P.wmat(wm, torch.zeros(N), len(taps), Cin, geglu=True)
             P.gemm(a, w, out_planes=P.planes(M, N // 2, tok), act=_lib.ACT_GEGLU, **kw)
@@ -95,16 +100,21 @@ def build(name, impl):
         ios["src"] = ("f32", src.ref, (rows, Cc)); ins["src"] = torch.randn(rows, Cc, generator=g)
         flops = 0.0
     pl = P.finish(ios)
-    return pl, ins, first, flops, sum(operand_bytes(o) for o in pl.ops[first:] if o["kind"] == "gemm")
+    arr = pl.resolve(1 << 32, 1 << 40)        # placeholder addresses: enough for the A-mode query
+    nbytes = sum(operand_bytes(o, _lib.gemm_a_mode(arr[i].u.gemm)) for i, o in enumerate(pl.ops) if i >= first and o["kind"] == "gemm")
+    return pl, ins, first, flops, nbytes
 
 
-def operand_bytes(o) -> int:
+def operand_bytes(o, amode=_lib.AMODE_GATHER) -> int:
     """Bytes one GEMM launch moves from L2 into shared memory: every 128-row tile gathers its A rows (K fp16 values per
-    plane) and receives its own copy of the [hi | lo] weight image of its N tile (Kpad x bn x 2 planes)."""
+    plane) and receives its own copy of the [hi | lo] weight image of its N tile (Kpad x bn x 2 planes).  In halo mode a
+    tile (64 columns wide) loads its 180-pixel halo once per 64-channel block instead of 9 x 128 pixel rows."""
     M = o["B"] * o["OH"] * o["OW"]
-    tiles_m, tiles_n = math.ceil(M / 128), math.ceil(o["N"] / o["bn"])
+    bn = 64 if amode == _lib.AMODE_HALO else o["bn"]       # the halo kernel runs 64-wide N tiles
+    tiles_m, tiles_n = math.ceil(M / 128), math.ceil(o["N"] / bn)
     ap = 2 if o["a_lo"] is not None else 1
-    return tiles_m * tiles_n * (128 * o["K"] * 2 * ap + o["bn"] * o["Kpad"] * 4)
+    a_rows = 180 * o["K"] // len(o["taps"]) if amode == _lib.AMODE_HALO else 128 * o["K"]
+    return tiles_m * tiles_n * (a_rows * 2 * ap + bn * o["Kpad"] * 4)
 
 
 def main():
