@@ -5,9 +5,10 @@ the nine taps from that copy through shifted shared-memory descriptors.
 The GPU cases run through test_gpu_kernel_matrix.test_gemm_matrix: the same float64 reference, error bounds and guard
 bands as every other GEMM variant.  They cover both tile shapes, with and without the nearest x2 upsample, one and two
 A planes, Cp of 64, 128, 256 and 640, batch 1
-and 16 with the batch modulo (x shared by the cond and uncond halves), the FAST, compact fp32 / plane and generic (NCHW)
-epilogues, ragged N tiles, and images of one tile row or column (every tile touches the zero border) up to several tiles
-per persistent CTA.  The CPU tests pin which descriptors take the halo path and that every other shape keeps the gather."""
+and 16 with the batch modulo (x shared by the cond and uncond halves), every epilogue body and store the halo path can
+take with one and with two A planes (FAST with a strided row vector and residual, compact fp32, compact and pair plane
+stores, and generic with NCHW, SiLU or alpha / accumulate), ragged N tiles, and images of one tile row or column (every
+tile touches the zero border) up to several tiles per persistent CTA.  The CPU tests pin which descriptors take the halo path and that every other shape keeps the gather."""
 import pytest
 
 from audioldm2_b200 import _lib, plan
@@ -32,6 +33,21 @@ HALO_CASES = {
     "halo_up_w8_a2_c64_bmod": dict(B=4, H=32, W=8, Cin=64, N=64, taps=T3, up=1, bmod=2, bn=64, out="planes"),
     # weights packed in 64-row tiles
     "halo_w16_a2_c64_bn64": dict(B=2, H=16, W=32, Cin=64, N=192, taps=T3, bn=64, res=True),
+    # FAST body with two A planes: the ResBlock's first convolution adds the timestep embedding, a row vector read at a
+    # column offset inside a row of every ResBlock's embeddings
+    "halo_w16_a2_c128_fast_emb": dict(B=4, H=8, W=32, Cin=128, N=128, taps=T3, bn=128, rowvec=True, ld_rowvec=1000,
+                                      rowvec_col=256, res=True, res_pad=4),
+    "halo_w8_a2_c64_fast_emb": dict(B=3, H=32, W=8, Cin=64, N=192, taps=T3, bn=128, rowvec=True, ld_rowvec=600,
+                                    rowvec_col=400, pad_cols=8),
+    "halo_up_w16_a2_c64_fast_emb": dict(B=2, H=16, W=32, Cin=64, N=128, taps=T3, up=1, bn=128, rowvec=True,
+                                        ld_rowvec=260, rowvec_col=132, res=True),
+    # GENERIC body: an activation; alpha / accumulate with a leading dimension the compact bodies cannot store
+    "halo_w16_a1_c64_silu": dict(B=2, H=8, W=16, Cin=64, N=128, taps=T3, bn=128, act=_lib.ACT_SILU, a_planes=1),
+    "halo_w8_a2_c128_alpha_acc": dict(B=2, H=16, W=8, Cin=128, N=128, taps=T3, bn=64, res=True, alpha=1 / 3,
+                                      accumulate=True, pad_cols=2),
+    # compact fp32 body with one A plane; pair plane stores with two
+    "halo_w16_a1_c128_f32n": dict(B=2, H=16, W=16, Cin=128, N=128, taps=T3, bn=128, a_planes=1),
+    "halo_w32_a2_c64_pair": dict(H=8, W=32, Cin=64, N=128, taps=T3, bn=128, out="planes", planes_out=1),
 }
 
 # shapes that must keep the gather: one property away from a halo case each
