@@ -17,7 +17,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libaldm_b200.so")
 SOURCES = ["gemm.cu", "prep.cu", "attention.cu", "elementwise.cu", "stft.cu", "program.cu", "engine_abi.cu", "microbench.cu",
-           "cond/seqgen.cu"]
+           "cond/seqgen.cu", "text/t5.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
@@ -25,7 +25,7 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-
 NVCC = shutil.which("nvcc") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
 
 MAX_TAPS = 16
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 # enums (keep in sync with the header; checked by tests/test_abi.py against the header text)
 GEMM_TC, GEMM_SIMT, GEMM_TC_V1 = 0, 1, 2
@@ -39,6 +39,7 @@ AMODE_GATHER, AMODE_HALO = 0, 1                                                 
 PREP_COPY, PREP_SILU, PREP_LRELU, PREP_GN, PREP_GN_SILU, PREP_LN = 0, 1, 2, 3, 4, 5
 OP_GEMM, OP_PREP, OP_ATTN, OP_SOFTMAX, OP_TEMB, OP_TRANSPOSE, OP_PACKB, OP_COPY = 1, 2, 3, 4, 5, 6, 7, 8
 OP_SEQ_ASSEMBLE, OP_KV_ATTN, OP_SEQ_FEEDBACK = 9, 10, 11
+OP_T5_EMBED, OP_T5_RMSNORM, OP_T5_ATTN, OP_T5_GATE = 12, 13, 14, 15
 
 
 class GemmDesc(C.Structure):
@@ -124,10 +125,32 @@ class SeqFeedbackDesc(C.Structure):
                 ("k", C.c_int32), ("gen_len", C.c_int32), ("eps", C.c_float)]
 
 
+class T5EmbedDesc(C.Structure):
+    _fields_ = [("ids", C.c_void_p), ("table", C.c_void_p), ("out", C.c_void_p), ("rows", C.c_int32), ("vocab", C.c_int32),
+                ("C", C.c_int32)]
+
+
+class T5RmsnormDesc(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("gamma", C.c_void_p), ("out_hi", C.c_void_p), ("out_lo", C.c_void_p),
+                ("out_f32", C.c_void_p), ("rows", C.c_int32), ("C", C.c_int32), ("ldo", C.c_int32), ("eps", C.c_float)]
+
+
+class T5AttnDesc(C.Structure):
+    _fields_ = [("qkv", C.c_void_p), ("bias", C.c_void_p), ("mask", C.c_void_p), ("out_hi", C.c_void_p), ("out_lo", C.c_void_p),
+                ("B", C.c_int32), ("L", C.c_int32), ("heads", C.c_int32), ("d_kv", C.c_int32), ("C", C.c_int32),
+                ("ld_qkv", C.c_int32), ("ldo", C.c_int32)]
+
+
+class T5GateDesc(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("out_hi", C.c_void_p), ("out_lo", C.c_void_p), ("sat", C.c_void_p),
+                ("rows", C.c_int32), ("F", C.c_int32), ("ld_x", C.c_int32), ("ldo", C.c_int32)]
+
+
 class _OpU(C.Union):
     _fields_ = [("gemm", GemmDesc), ("prep", PrepDesc), ("attn", AttnDesc), ("softmax", _Softmax),
                 ("temb", _Temb), ("transpose", _Transpose), ("packb", _PackB), ("copy", _Copy),
-                ("seq_assemble", SeqAssembleDesc), ("kv_attn", KvAttnDesc), ("seq_feedback", SeqFeedbackDesc)]
+                ("seq_assemble", SeqAssembleDesc), ("kv_attn", KvAttnDesc), ("seq_feedback", SeqFeedbackDesc),
+                ("t5_embed", T5EmbedDesc), ("t5_rmsnorm", T5RmsnormDesc), ("t5_attn", T5AttnDesc), ("t5_gate", T5GateDesc)]
 
 
 class Op(C.Structure):
@@ -207,6 +230,10 @@ def lib() -> C.CDLL:
         "aldm_kv_attention": (i32, [C.POINTER(KvAttnDesc), vp]),
         "aldm_seq_assemble": (i32, [C.POINTER(SeqAssembleDesc), vp]),
         "aldm_seq_feedback": (i32, [C.POINTER(SeqFeedbackDesc), vp]),
+        "aldm_t5_embed": (i32, [C.POINTER(T5EmbedDesc), vp]),
+        "aldm_t5_rmsnorm": (i32, [C.POINTER(T5RmsnormDesc), vp]),
+        "aldm_t5_attention": (i32, [C.POINTER(T5AttnDesc), vp]),
+        "aldm_t5_gate": (i32, [C.POINTER(T5GateDesc), vp]),
         "aldm_softmax_rows": (i32, [vp, i32, i32, f32, vp, vp, vp]),
         "aldm_timestep_embedding": (i32, [vp, i32, i32, vp, vp, vp, vp]),
         "aldm_ddim_step": (i32, [vp, vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, vp]),
@@ -257,6 +284,7 @@ def lib() -> C.CDLL:
 
 EXPORTED = ["aldm_gemm", "aldm_gemm_variant", "aldm_gemm_a_mode", "aldm_prep", "aldm_pack_b", "aldm_attention", "aldm_softmax_rows",
             "aldm_kv_attention", "aldm_seq_assemble", "aldm_seq_feedback",
+            "aldm_t5_embed", "aldm_t5_rmsnorm", "aldm_t5_attention", "aldm_t5_gate",
             "aldm_timestep_embedding", "aldm_ddim_step", "aldm_masked_blend", "aldm_transpose_chw",
             "aldm_posterior_sample", "aldm_stft_mel", "aldm_program_create", "aldm_program_run",
             "aldm_program_run_range", "aldm_program_capture", "aldm_program_replay",

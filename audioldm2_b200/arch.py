@@ -388,3 +388,42 @@ def has_seqgen(cfg: dict) -> bool:
     (phoneme-conditioned 512-token generation, not built here) have no such stage."""
     dims = [c for c in (cfg["unet"].get("context_dim") or []) if c is not None]
     return dims[:2] == [768, 1024] and "-speech-" not in cfg.get("name", "")
+
+
+# --------------------------------------------------------------------------------------
+# Flan-T5-large text encoder (FlanT5HiddenState, encoders/modules.py:113-198: T5EncoderModel(T5Config.from_pretrained(
+# "google/flan-t5-large")), run in fp32): 24 blocks, width 1024, 16 heads of 64, gated-GELU feed-forward of 2816 with
+# gelu_new, RMSNorm eps 1e-6, 32 bidirectional relative-position buckets up to distance 128 (layer 0's table, shared by
+# every layer), no biases, unscaled embedding.  The tokenizer (max_length 128, pad id 0, "" -> [1]) stays on the host.
+# --------------------------------------------------------------------------------------
+
+T5 = dict(d_model=1024, n_head=16, d_kv=64, d_ff=2816, n_layer=24, vocab=32128, eps=1e-6, num_buckets=32,
+          max_distance=128, max_len=128, pad_id=0, eos_id=1)
+
+
+def t5_param_shapes(n_layer: int = 24, with_embed_tokens: bool = True) -> Dict[str, Tuple[int, ...]]:
+    """name -> shape of HF ``T5EncoderModel``'s state dict (relative to ``cond_stage_models.<i>.model.``).
+    ``encoder.embed_tokens.weight`` is tied to ``shared.weight``."""
+    C, F, H, V = T5["d_model"], T5["d_ff"], T5["n_head"], T5["vocab"]
+    P: Dict[str, Tuple[int, ...]] = {"shared.weight": (V, C)}
+    if with_embed_tokens:
+        P["encoder.embed_tokens.weight"] = (V, C)
+    for i in range(n_layer):
+        b = f"encoder.block.{i}.layer"
+        for n in ("q", "k", "v", "o"):
+            P[f"{b}.0.SelfAttention.{n}.weight"] = (C, C)
+        if i == 0:
+            P[f"{b}.0.SelfAttention.relative_attention_bias.weight"] = (T5["num_buckets"], H)
+        P[f"{b}.0.layer_norm.weight"] = (C,)
+        P[f"{b}.1.DenseReluDense.wi_0.weight"] = (F, C)
+        P[f"{b}.1.DenseReluDense.wi_1.weight"] = (F, C)
+        P[f"{b}.1.DenseReluDense.wo.weight"] = (C, F)
+        P[f"{b}.1.layer_norm.weight"] = (C,)
+    P["encoder.final_layer_norm.weight"] = (C,)
+    return P
+
+
+def has_t5(cfg: dict) -> bool:
+    """Configs whose UNet reads Flan-T5 states (a 1024-wide context): audioldm2-full / -large (next to the AudioMAE
+    tokens) and the *_t5 models."""
+    return 1024 in [c for c in (cfg["unet"].get("context_dim") or []) if c is not None]

@@ -47,6 +47,10 @@ int attention_launch(const aldm_attn_desc& d, cudaStream_t st);
 int kv_attention_launch(const aldm_kv_attn_desc& d, cudaStream_t st);
 int seq_assemble_launch(const aldm_seq_assemble_desc& d, cudaStream_t st);
 int seq_feedback_launch(const aldm_seq_feedback_desc& d, cudaStream_t st);
+int t5_embed_launch(const aldm_t5_embed_desc& d, cudaStream_t st);
+int t5_rmsnorm_launch(const aldm_t5_rmsnorm_desc& d, cudaStream_t st);
+int t5_attention_launch(const aldm_t5_attn_desc& d, cudaStream_t st);
+int t5_gate_launch(const aldm_t5_gate_desc& d, cudaStream_t st);
 
 }  // namespace aldm
 
@@ -78,6 +82,10 @@ static int run_op(const aldm_op& op, cudaStream_t st) {
     case ALDM_OP_SEQ_ASSEMBLE: return seq_assemble_launch(op.u.seq_assemble, st);
     case ALDM_OP_KV_ATTN: return kv_attention_launch(op.u.kv_attn, st);
     case ALDM_OP_SEQ_FEEDBACK: return seq_feedback_launch(op.u.seq_feedback, st);
+    case ALDM_OP_T5_EMBED: return t5_embed_launch(op.u.t5_embed, st);
+    case ALDM_OP_T5_RMSNORM: return t5_rmsnorm_launch(op.u.t5_rmsnorm, st);
+    case ALDM_OP_T5_ATTN: return t5_attention_launch(op.u.t5_attn, st);
+    case ALDM_OP_T5_GATE: return t5_gate_launch(op.u.t5_gate, st);
     case ALDM_OP_COPY:
       ALDM_CHECK_CUDA(cudaMemcpyAsync(op.u.copy.dst, op.u.copy.src, (size_t)op.u.copy.bytes, cudaMemcpyDeviceToDevice, st));
       return ALDM_OK;

@@ -15,7 +15,7 @@ import torch
 from . import _lib
 from .plan import Plan
 
-_TORCH_DT = {"f32": torch.float32, "i64": torch.int64}
+_TORCH_DT = {"f32": torch.float32, "i64": torch.int64, "i32": torch.int32}
 
 
 def _stream_ptr() -> int:

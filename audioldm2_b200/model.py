@@ -64,6 +64,24 @@ def split_seqgen_state_dict(state_dict: Dict[str, torch.Tensor], index: int = 0)
     return out
 
 
+def split_t5_state_dict(state_dict: Dict[str, torch.Tensor], prefix: str) -> Dict[str, torch.Tensor]:
+    """The Flan-T5 encoder's weights from a reference checkpoint: the keys under ``prefix`` (a ``T5EncoderModel``, e.g.
+    ``cond_stage_models.1.model.``), named and shaped as arch.t5_param_shapes.  ``encoder.embed_tokens.weight`` (tied to
+    ``shared.weight``) is optional and not returned.  Raises KeyError for a missing key, ValueError for a wrong shape."""
+    n_layer = len([k for k in state_dict if k.startswith(prefix + "encoder.block.") and k.endswith(".layer.0.layer_norm.weight")])
+    if n_layer == 0:
+        raise KeyError(f"checkpoint has no T5 encoder blocks under {prefix}encoder.block.")
+    out = {}
+    for k, shp in arch.t5_param_shapes(n_layer, with_embed_tokens=False).items():
+        v = state_dict.get(prefix + k)
+        if v is None:
+            raise KeyError(f"checkpoint has no {prefix + k} (needed by the Flan-T5 encoder)")
+        if tuple(v.shape) != tuple(shp):
+            raise ValueError(f"{prefix + k}: shape {tuple(v.shape)}, expected {shp}")
+        out[k] = v
+    return out
+
+
 def reorder_cond_dict(cond_dict: dict, conditioning_key: Sequence[str]) -> dict:
     """LatentDiffusion.reorder_cond_dict (ddpm.py:1028-1032): the UNet consumes the conditions in the order of
     ``conditioning_key`` (the config's list), not in the dict's insertion order."""

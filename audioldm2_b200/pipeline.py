@@ -11,6 +11,10 @@ network.  What differs, by design of this tier:
   or, for the sequence-generation models (audioldm2-full / -large), the encoder outputs ``film_clap_cond1`` [B, 1, 512]
   and ``crossattn_flan_t5`` [h [B, L, 1024], mask [B, L]]: the AudioMAE tokens are then generated natively by GPT-2
   (seqgen.NativeAudioMAEGenerator), on the B prompts before the n_gen tiling as in generate_batch (ddpm.py:1500-1523);
+  or, for every model with a Flan-T5 context (audioldm2-full / -large, the *_t5 models), the tokenizer's output under the
+  reference's own key, ``crossattn_flan_t5`` = [input_ids (integer) [B, L], attention_mask [B, L]] (plus
+  ``film_clap_cond1`` for the sequence-generation models): the T5 states are then encoded natively
+  (t5.NativeFlanT5Encoder) before anything else, in the conditional and the unconditional dict alike;
 * candidate re-ranking (ddpm.py:1554-1568) uses ``latent_diffusion.ranker(waveform [n,1,L], texts) -> similarity [n]``
   (the reference's ``clap.cos_similarity``); without one the first candidate of each prompt is returned and a
   warning says so;
@@ -69,6 +73,64 @@ class SyntheticEncoderOutputs:
                     (v.expand(n, *v.shape[1:]).contiguous() if torch.is_tensor(v) else v)) for k, v in u.items()}
 
 
+class SyntheticTokenIds:
+    """Seeded tokenizer output for every model with a Flan-T5 context (opt-in): ``crossattn_flan_t5`` = [ids, mask] with
+    per-row token counts (row i holds ``lens[i % len]`` tokens ending in EOS, L = the longest: padding=True), and for the
+    sequence-generation models an L2-normalised CLAP embedding [B, 1, 512].  The unconditional branch is the tokenization
+    of "" ([[1]] on every row) next to zero AudioMAE tokens where the model has them: the same rows whatever the row
+    count, as in the reference."""
+
+    def __init__(self, cfg: dict, seed: int = 79, lens=(32, 19, 7), device="cpu"):
+        if not arch.has_t5(cfg):
+            raise ValueError(f"{cfg.get('name')}: token ids need a Flan-T5 context, which this model has not")
+        self.cfg, self.seed, self.lens, self.device = cfg, seed, tuple(lens), device
+
+    def cond(self, batch: dict) -> dict:
+        n = len(batch["text"])
+        ids, mask = synth.token_ids([self.lens[i % len(self.lens)] for i in range(n)], seed=self.seed, device=self.device)
+        out = {}
+        if arch.has_seqgen(self.cfg):
+            g = torch.Generator(device="cpu"); g.manual_seed(self.seed + 1)
+            clap = torch.randn(n, 1, 512, generator=g)
+            out["film_clap_cond1"] = (clap / clap.norm(dim=-1, keepdim=True)).to(self.device)
+        out["crossattn_flan_t5"] = [ids, mask]
+        return out
+
+    def uncond(self, n: int) -> dict:
+        one = torch.ones(n, 1, device=self.device)
+        out = {}
+        if arch.has_seqgen(self.cfg):                 # zero AudioMAE tokens (encoders/modules.py:476-479)
+            out["crossattn_audiomae_generated"] = [torch.zeros(n, 8, 768, device=self.device), torch.ones(n, 8, device=self.device)]
+        out["crossattn_flan_t5"] = [(one * arch.T5["eos_id"]).long(), one]
+        return out
+
+
+def is_token_level(cond) -> bool:
+    """The Flan-T5 entry holds the tokenizer's output (integer ids) rather than hidden states."""
+    if not isinstance(cond, dict) or not isinstance(cond.get("crossattn_flan_t5"), (list, tuple)):
+        return False
+    ids = cond["crossattn_flan_t5"][0]
+    return torch.is_tensor(ids) and not ids.dtype.is_floating_point and not ids.dtype.is_complex
+
+
+def encode_tokens(cfg: dict, cond: dict, encoder: Callable[[], object], unconditional: bool = False) -> dict:
+    """Replace token-level ``crossattn_flan_t5`` = [ids, mask] by [encoder().encode(ids, mask), mask.float()] (every other
+    entry is kept, in order); anything else is returned as it is and the encoder is never built.  In the unconditional
+    dict, the tokenization of "" ([[1]] on every row, mask 1) goes through ``encoder().unconditional(n)``, computed once
+    and cached like the reference's T5("") (encoders/modules.py:139-154)."""
+    if not is_token_level(cond):
+        return cond
+    if not arch.has_t5(cfg):
+        raise ValueError(f"{cfg.get('name')} has no Flan-T5 context: token ids under crossattn_flan_t5 do not apply")
+    ids, mask = cond["crossattn_flan_t5"]
+    enc = encoder()
+    if unconditional and ids.shape[1] == 1 and bool((ids == arch.T5["eos_id"]).all()) and bool((mask == 1).all()):
+        h = enc.unconditional(ids.shape[0])
+    else:
+        h = enc.encode(ids, mask)
+    return {k: ([h, mask.float().to(h.device)] if k == "crossattn_flan_t5" else v) for k, v in cond.items()}
+
+
 def is_encoder_level(cond: dict) -> bool:
     """Encoder outputs rather than UNet-boundary conditioning: CLAP + Flan-T5 present, no AudioMAE tokens, not unpacked."""
     return isinstance(cond, dict) and "film_clap_cond1" in cond and "crossattn_flan_t5" in cond and \
@@ -119,7 +181,10 @@ class NativeAudioLDM2:
     ``generate_batch_masked``, ``latent_t_size``) over per-shape native engines."""
 
     def __init__(self, cfg: dict, unet_sd, vae_sd, vocoder_sd, device, scale_factor: float = 1.0, ctx_max_len=None,
-                 cond_provider=None, ranker: Optional[Callable] = None, seqgen_sd=None, **engine_kw):
+                 cond_provider=None, ranker: Optional[Callable] = None, seqgen_sd=None, t5_sd=None, t5_uncond_sd=None,
+                 **engine_kw):
+        """``t5_sd`` / ``t5_uncond_sd``: the Flan-T5 weights of the conditional and of the unconditional branch (or callables
+        that return them, for weights made on first use); ``t5_uncond_sd`` None means the same weights."""
         self.cfg, self.device = cfg, torch.device(device)
         self._sd = (unet_sd, vae_sd, vocoder_sd)
         self.scale_factor = scale_factor
@@ -132,6 +197,8 @@ class NativeAudioLDM2:
         self._pinned: Dict[Tuple[int, ...], torch.Tensor] = {}
         self._seqgen_sd = seqgen_sd
         self._seqgen = None
+        self._t5_sd, self._t5_uncond_sd = t5_sd, t5_uncond_sd
+        self._t5 = None
 
     # ---- AudioMAE token generator (built on first use: UNet-boundary providers never pay for it) ----------------------
     def seqgen(self):
@@ -143,10 +210,36 @@ class NativeAudioLDM2:
             self._seqgen = NativeAudioMAEGenerator(self._seqgen_sd, self.device)
         return self._seqgen
 
+    # ---- Flan-T5 encoder (built on first token-level use) ---------------------------------------------------
+    def t5_encoders(self):
+        """(conditional, unconditional) native encoders.  One packed arena serves both when the two weight sets are
+        equal (the checkpoint holds two frozen copies of the same pretrained encoder), otherwise each has its own."""
+        if self._t5 is None:
+            if self._t5_sd is None:
+                raise ValueError("token-level conditioning needs the Flan-T5 weights, which this model was built without")
+            from .t5 import NativeFlanT5Encoder
+            get = lambda w: w() if callable(w) else w
+            sd_c = get(self._t5_sd)
+            enc_c = NativeFlanT5Encoder(sd_c, self.device)
+            enc_u = enc_c
+            if self._t5_uncond_sd is not None:
+                sd_u = get(self._t5_uncond_sd)
+                same = sd_u is sd_c or (set(sd_u) == set(sd_c) and all(torch.equal(sd_u[k], sd_c[k]) for k in sd_c))
+                if not same:
+                    enc_u = NativeFlanT5Encoder(sd_u, self.device)
+            self._t5 = (enc_c, enc_u)
+        return self._t5
+
     def conditioning(self, batch) -> dict:
-        """The provider's conditioning of the call's B prompts, with the AudioMAE tokens generated when it holds
-        encoder outputs."""
-        return route_conditioning(self.cfg, self.cond_provider.cond(batch), self.seqgen)
+        """The provider's conditioning of the call's B prompts: token ids encoded by Flan-T5, then the AudioMAE tokens
+        generated when it holds encoder outputs."""
+        cond = encode_tokens(self.cfg, self.cond_provider.cond(batch), lambda: self.t5_encoders()[0])
+        return route_conditioning(self.cfg, cond, self.seqgen)
+
+    def unconditioning(self, n: int, uncond=None) -> dict:
+        """The unconditional branch (the provider's unless given), with token ids encoded by the unconditional encoder."""
+        u = self.cond_provider.uncond(n) if uncond is None else uncond
+        return encode_tokens(self.cfg, u, lambda: self.t5_encoders()[1], unconditional=True)
 
     # ---- engines -------------------------------------------------------------------------------------
     def engine(self, Bl: int, latent_t: Optional[int] = None, with_encoder: bool = False) -> model.NativeLatentDiffusion:
@@ -244,8 +337,8 @@ class NativeAudioLDM2:
             mask[:, :, int(F_ * fmask[0]):int(F_ * fmask[1])] = 0
             mask = mask[:, None].contiguous()
         cond = _tile(cond_rows if cond_rows is not None else self.conditioning(batch), n_gen)
-        if guidance != 1.0 and uncond is None:
-            uncond = self.cond_provider.uncond(Bl)                                        # ddpm.py:1529-1536
+        if guidance != 1.0:
+            uncond = self.unconditioning(Bl, uncond)                                      # ddpm.py:1529-1536
         texts = list(batch["text"]) * n_gen
         wave = eng.generate_waveform(cond, uncond, ddim_steps=ddim_steps, guidance=guidance, eta=ddim_eta, mask=mask, x0=x0,
                                      x_T=x_T, noise_fn=noise_fn)
@@ -262,11 +355,17 @@ class NativeAudioLDM2:
 
 def build_model(ckpt_path=None, config=None, device=None, model_name="audioldm2-full", *, synthetic: Optional[bool] = None,
                 cond_provider=None, ranker: Optional[Callable] = None, t5_len: int = 32, ctx_max_len=None, seqgen_index: int = 0,
-                **engine_kw):
+                t5_index: Optional[int] = None, **engine_kw):
     """pipeline.py:142-179.  ``ckpt_path`` is a reference ``<model_name>.pth`` (``["state_dict"]``, key layout of SURVEY.md
     8b); without it (no network here, utils.py:209-219) the seeded synthetic checkpoint is used.  For audioldm2-full / -large
     the AudioMAE generator's weights are taken too (``cond_stage_models.<seqgen_index>.``), for encoder-level providers.  Engines are planned lazily
-    for the latent batch of each call (``batchsize * n_candidate_gen_per_text``)."""
+    for the latent batch of each call (``batchsize * n_candidate_gen_per_text``).
+
+    The Flan-T5 weights, for token-level providers: audioldm2-full / -large encode the conditional branch with the
+    generator's inner T5 (``cond_stage_models.<seqgen_index>.cond_stage_models.<t5_index>.model.``, t5_index 1 by default:
+    get_input skips a key an earlier model already produced, ddpm.py:861-862) and T5("") with the top-level copy
+    (``cond_stage_models.<t5_index>.model.``, ddpm.py:1529-1533); the *_t5 models use ``cond_stage_models.<t5_index>``
+    (default 0) for both.  Synthetic weights are generated on first token-level use."""
     if device is None or device == "auto":
         device = torch.device("cuda:0")          # the native path has no CPU / MPS fallback
     cfg = arch.model_config(model_name) if config is None else config
@@ -279,6 +378,8 @@ def build_model(ckpt_path=None, config=None, device=None, model_name="audioldm2-
         un, vae, voc, sf = synth.unet_state_dict(cfg["unet"]), synth.vae_state_dict(cfg["vae"]), \
             synth.vocoder_state_dict(cfg["vocoder"]), 1.0
         seq = synth.seqgen_state_dict() if arch.has_seqgen(cfg) else None
+        t5c = synth.t5_state_dict if arch.has_t5(cfg) else None
+        t5u = None
         if ctx_max_len is None:
             n_cross = len([c for c in cfg["unet"]["context_dim"] if c is not None])
             ctx_max_len = (8, t5_len) if n_cross > 1 else (t5_len,)
@@ -286,7 +387,15 @@ def build_model(ckpt_path=None, config=None, device=None, model_name="audioldm2-
         sd = torch.load(ckpt_path, map_location="cpu")["state_dict"]                      # pipeline.py:172
         un, vae, voc, sf = model.split_state_dict(sd)
         seq = model.split_seqgen_state_dict(sd, seqgen_index) if arch.has_seqgen(cfg) else None
+        t5c = t5u = None
+        if arch.has_seqgen(cfg):
+            j = 1 if t5_index is None else t5_index
+            t5c = model.split_t5_state_dict(sd, f"cond_stage_models.{seqgen_index}.cond_stage_models.{j}.model.")
+            t5u = model.split_t5_state_dict(sd, f"cond_stage_models.{j}.model.")
+        elif arch.has_t5(cfg):
+            t5c = model.split_t5_state_dict(sd, f"cond_stage_models.{t5_index or 0}.model.")
     ld = NativeAudioLDM2(cfg, un, vae, voc, device, scale_factor=sf, ctx_max_len=ctx_max_len, seqgen_sd=seq,
+                         t5_sd=t5c, t5_uncond_sd=t5u,
                          cond_provider=cond_provider or SyntheticConditioning(cfg, t5_len=t5_len, device=device), ranker=ranker,
                          **engine_kw)
     ld.model_name = model_name

@@ -239,6 +239,30 @@ class Plan:
                 for name in ("B", "nq", "C", "pos", "k", "gen_len"):
                     setattr(a, name, int(o[name]))
                 a.eps = float(o["eps"])
+            elif k == "t5_embed":
+                op.kind = _lib.OP_T5_EMBED
+                a = op.u.t5_embed
+                a.ids, a.table, a.out = P(o["ids"]), P(o["table"]), P(o["out"])
+                a.rows, a.vocab, a.C = int(o["rows"]), int(o["vocab"]), int(o["C"])
+            elif k == "t5_rmsnorm":
+                op.kind = _lib.OP_T5_RMSNORM
+                a = op.u.t5_rmsnorm
+                for name in ("x", "gamma", "out_hi", "out_lo", "out_f32"):
+                    setattr(a, name, P(o.get(name)))
+                a.rows, a.C, a.ldo, a.eps = int(o["rows"]), int(o["C"]), int(o["ldo"]), float(o["eps"])
+            elif k == "t5_attn":
+                op.kind = _lib.OP_T5_ATTN
+                a = op.u.t5_attn
+                for name in ("qkv", "bias", "mask", "out_hi", "out_lo"):
+                    setattr(a, name, P(o.get(name)))
+                for name in ("B", "L", "heads", "d_kv", "C", "ld_qkv", "ldo"):
+                    setattr(a, name, int(o[name]))
+            elif k == "t5_gate":
+                op.kind = _lib.OP_T5_GATE
+                a = op.u.t5_gate
+                for name in ("x", "out_hi", "out_lo", "sat"):
+                    setattr(a, name, P(o.get(name)))
+                a.rows, a.F, a.ld_x, a.ldo = int(o["rows"]), int(o["F"]), int(o["ld_x"]), int(o["ldo"])
             elif k == "copy":
                 op.kind = _lib.OP_COPY
                 c = op.u.copy
@@ -1070,5 +1094,148 @@ def build_seqgen(sd: Optional[Dict[str, torch.Tensor]], batch: int, t5_len: int,
     P.mark("end")
     assert P.arena.size == 0, "generator plans reference the shared weight arena only"
     pl = P.finish(io, meta=dict(B=B, L=L, P=Pn, lmax=lmax, gen_len=gen_len, n_layer=W.n_layer))
+    pl.arena = W.arena
+    return pl
+
+
+# ==============================================================================================
+# Flan-T5 encoder from token ids (FlanT5HiddenState.encode_text, encoders/modules.py:173-198; HF T5EncoderModel)
+# ==============================================================================================
+T5_BN = 64           # N tile of every encoder GEMM: the same packed weights serve 1 to 1024 rows (N = 1024 gives 16 tiles
+                     # per 128-row block; split-K fills the machine for the short-M wo GEMMs)
+
+
+def t5_relative_position_bucket(relative_position: torch.Tensor, num_buckets: int = 32, max_distance: int = 128) -> torch.Tensor:
+    """T5Attention._relative_position_bucket with bidirectional=True (the encoder), restated with the same torch
+    operations in the same order (so the same float32 logs decide the boundaries): offset j - i -> bucket in [0, 32)."""
+    num_buckets //= 2
+    buckets = (relative_position > 0).to(torch.long) * num_buckets
+    rp = torch.abs(relative_position)
+    max_exact = num_buckets // 2
+    is_small = rp < max_exact
+    large = max_exact + (torch.log(rp.float() / max_exact) / math.log(max_distance / max_exact)
+                         * (num_buckets - max_exact)).to(torch.long)
+    large = torch.min(large, torch.full_like(large, num_buckets - 1))
+    return buckets + torch.where(is_small, rp, large)
+
+
+def t5_bias_table(rel_bias: torch.Tensor) -> torch.Tensor:
+    """relative_attention_bias.weight [32, heads] -> [heads, 255]: the bias of offsets j - i = -127 .. 127, the only
+    thing the attention kernel reads (it indexes column j - i + 127).  Built here once so that no device-side log can
+    move a bucket boundary."""
+    L = arch.T5["max_len"]
+    off = torch.arange(-(L - 1), L)
+    b = t5_relative_position_bucket(off, arch.T5["num_buckets"], arch.T5["max_distance"])
+    return rel_bias.float()[b].t().contiguous()
+
+
+@dataclass
+class T5Weights:
+    """The encoder's weight arena, packed once and shared by the plans of every (batch, length)."""
+    arena: torch.Tensor
+    n_layer: int
+    refs: Dict[str, object]
+
+
+def pack_t5_weights(sd: Dict[str, torch.Tensor], **pk) -> T5Weights:
+    """Weights of split_t5_state_dict / synth.t5_state_dict -> arena: shared.weight in fp32 (the embedding gather), the
+    [heads, 255] bias table, the RMSNorm weights, and per block the fused [q | k | v], o, [wi_0 | wi_1] and wo matrices
+    as two-plane tile images."""
+    P = Planner(**pk)
+    n_layer = len([k for k in sd if k.startswith("encoder.block.") and k.endswith(".layer.0.layer_norm.weight")])
+    if n_layer == 0:
+        raise KeyError("state dict holds no T5 blocks (encoder.block.<i>.*)")
+
+    def lin(ws) -> WMat:
+        wm, taps, cp = packing.conv_weight_matrix(torch.cat([w.float() for w in ws], 0))
+        return P.wmat(wm, None, taps, cp, bn=T5_BN)
+
+    r: Dict[str, object] = {
+        "table": P.vec(sd["shared.weight"]),
+        "bias": P.vec(t5_bias_table(sd["encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight"])),
+        "final": P.vec(sd["encoder.final_layer_norm.weight"]),
+    }
+    for i in range(n_layer):
+        b = f"encoder.block.{i}.layer"
+        a = f"{b}.0.SelfAttention"
+        f = f"{b}.1.DenseReluDense"
+        r[f"{i}.ln0"] = P.vec(sd[f"{b}.0.layer_norm.weight"])
+        r[f"{i}.ln1"] = P.vec(sd[f"{b}.1.layer_norm.weight"])
+        r[f"{i}.qkv"] = lin([sd[f"{a}.q.weight"], sd[f"{a}.k.weight"], sd[f"{a}.v.weight"]])
+        r[f"{i}.o"] = lin([sd[f"{a}.o.weight"]])
+        r[f"{i}.wi"] = lin([sd[f"{f}.wi_0.weight"], sd[f"{f}.wi_1.weight"]])
+        r[f"{i}.wo"] = lin([sd[f"{f}.wo.weight"]])
+    return T5Weights(P.arena.build(), n_layer, r)
+
+
+def build_t5(sd: Optional[Dict[str, torch.Tensor]], batch: int, length: int, weights: Optional[T5Weights] = None,
+             **pk) -> Plan:
+    """T5EncoderModel(input_ids, attention_mask).last_hidden_state for one (batch B, length L <= 128), in fp32.
+
+    io: ids [B, L] int64, mask [B, L] fp32 (1 = token) in; hidden [B, L, 1024] fp32 out; sat [n_layer] int32, the
+    per-block count of gated-GELU values beyond the fp16 range (zero unless a run saturated; the caller reads and
+    clears it).  Launches: the embedding, 8 per block (RMSNorm, QKV GEMM, attention, o GEMM + residual, RMSNorm,
+    [wi_0 | wi_1] GEMM, gate, wo GEMM + residual) and final_layer_norm.  Marks "begin", "end".  The plan references
+    the arena of ``weights`` (packed from ``sd`` when None)."""
+    W = weights if weights is not None else pack_t5_weights(sd, **pk)
+    P = Planner(**pk)
+    B, L = int(batch), int(length)
+    if B < 1 or not 1 <= L <= arch.T5["max_len"]:
+        raise ValueError(f"t5: batch {B}, length {L} (1 .. {arch.T5['max_len']} tokens)")
+    C, H, Dk, Fd = arch.T5["d_model"], arch.T5["n_head"], arch.T5["d_kv"], arch.T5["d_ff"]
+    eps = arch.T5["eps"]
+    R = B * L
+    r = W.refs
+    ids = P.raw(R * 8)
+    mask = P.raw(R * 4)
+    hidden = P.raw(R * C * 4)
+    sat = P.raw(W.n_layer * 4)
+    io = dict(ids=("i64", ids, (B, L)), mask=("f32", mask, (B, L)), hidden=("f32", hidden, (B, L, C)),
+              sat=("i32", sat, (W.n_layer,)))
+
+    P.mark("begin")
+    P.tag = 0
+    x = P.f32(R, C)
+    P.ops.append(dict(kind="t5_embed", tag=0, ids=ids, table=r["table"], out=x.ref, rows=R, vocab=arch.T5["vocab"], C=C))
+
+    def rms(src: F32, gamma: Ref) -> Planes:
+        out = P.planes(R, C)
+        P.ops.append(dict(kind="t5_rmsnorm", tag=P.tag, x=src.ref, gamma=gamma, out_hi=out.hi, out_lo=out.lo, out_f32=None,
+                          rows=R, C=C, ldo=out.Cp, eps=eps))
+        return out
+
+    for i in range(W.n_layer):
+        P.tag = 1 + i
+        # T5LayerSelfAttention: x + o(attn(rms(x)))
+        a = rms(x, r[f"{i}.ln0"])
+        qkv = P.f32(R, 3 * C)
+        P.gemm(a, r[f"{i}.qkv"], B=1, H=R, out=qkv)
+        P.free(a)
+        o = P.planes(R, C)
+        P.ops.append(dict(kind="t5_attn", tag=P.tag, qkv=qkv.ref, bias=r["bias"], mask=mask, out_hi=o.hi, out_lo=o.lo, B=B, L=L,
+                          heads=H, d_kv=Dk, C=C, ld_qkv=3 * C, ldo=o.Cp))
+        P.free(qkv)
+        x2 = P.f32(R, C)
+        P.gemm(o, r[f"{i}.o"], B=1, H=R, out=x2, res=x)
+        P.free(o, x)
+        # T5LayerFF (gated-gelu): x + wo(gelu_new(wi_0(rms(x))) * wi_1(rms(x)))
+        a = rms(x2, r[f"{i}.ln1"])
+        hf = P.f32(R, 2 * Fd)
+        P.gemm(a, r[f"{i}.wi"], B=1, H=R, out=hf)
+        P.free(a)
+        g = P.planes(R, Fd)
+        P.ops.append(dict(kind="t5_gate", tag=P.tag, x=hf.ref, out_hi=g.hi, out_lo=g.lo, sat=sat + 4 * i, rows=R, F=Fd,
+                          ld_x=2 * Fd, ldo=g.Cp))
+        P.free(hf)
+        x = P.f32(R, C)
+        P.gemm(g, r[f"{i}.wo"], B=1, H=R, out=x, res=x2)
+        P.free(g, x2)
+    P.tag = 1 + W.n_layer
+    P.ops.append(dict(kind="t5_rmsnorm", tag=P.tag, x=x.ref, gamma=r["final"], out_hi=None, out_lo=None, out_f32=hidden,
+                      rows=R, C=C, ldo=C, eps=eps))
+    P.free(x)
+    P.mark("end")
+    assert P.arena.size == 0, "encoder plans reference the shared weight arena only"
+    pl = P.finish(io, meta=dict(B=B, L=L, n_layer=W.n_layer))
     pl.arena = W.arena
     return pl

@@ -97,6 +97,50 @@ def seqgen_state_dict(seed: int = 1237, n_layer: int = 12) -> Dict[str, torch.Te
     return out
 
 
+def t5_state_dict(seed: int = 1238, n_layer: int = 24) -> Dict[str, torch.Tensor]:
+    """Seeded Flan-T5 encoder checkpoint (HF ``T5EncoderModel`` keys, arch.t5_param_shapes).  Not ``_fill``: the gains
+    follow HF's T5 initialisation so that the unscaled logits stay O(1) -- q ~ N(0, 1/(1024 * 64)), k / v ~ N(0, 1/1024)
+    -- and the two residual projections (o, wo) are scaled by 1/sqrt(2 n_layer) so that the residual stream stays O(1)
+    over all blocks; the embedding and the relative-position bias are N(0, 1), RMSNorm weights 1 + 0.1 N(0, 1).
+    ``encoder.embed_tokens.weight`` is ``shared.weight`` (tied), as in the module's state dict."""
+    C, Dk = arch.T5["d_model"], arch.T5["d_kv"]
+    shapes = arch.t5_param_shapes(n_layer, with_embed_tokens=False)
+    g = torch.Generator(device="cpu")
+    g.manual_seed(seed)
+    res = 1.0 / math.sqrt(2 * n_layer)
+    out = {}
+    for name in sorted(shapes):
+        shp = shapes[name]
+        t = torch.randn(shp, generator=g)
+        if name == "shared.weight" or name.endswith("relative_attention_bias.weight"):
+            pass
+        elif len(shp) == 1:
+            t = 1.0 + 0.1 * t
+        elif name.endswith(".q.weight"):
+            t = t / math.sqrt(C * Dk)
+        elif name.endswith((".o.weight", ".wo.weight")):
+            t = t * (res / math.sqrt(shp[1]))
+        else:
+            t = t / math.sqrt(shp[1])
+        out[name] = t.contiguous()
+    out["encoder.embed_tokens.weight"] = out["shared.weight"]
+    return out
+
+
+def token_ids(lens, seed: int = 79, device="cpu"):
+    """Seeded tokenizer output: ids [B, L] int64 and attention_mask [B, L] float, L = max(lens) (padding=True).  Row i
+    holds lens[i] - 1 ids drawn from [2, vocab), then EOS (1), then pad (0) -- the layout of a T5 tokenization."""
+    g = torch.Generator(device="cpu"); g.manual_seed(seed)
+    lens = [int(n) for n in lens]
+    assert min(lens) >= 1 and max(lens) <= arch.T5["max_len"]
+    L = max(lens)
+    ids = torch.randint(2, arch.T5["vocab"], (len(lens), L), generator=g)
+    mask = (torch.arange(L)[None, :] < torch.tensor(lens)[:, None])
+    ids[torch.arange(len(lens)), torch.tensor(lens) - 1] = arch.T5["eos_id"]
+    ids = torch.where(mask, ids, torch.full_like(ids, arch.T5["pad_id"]))
+    return ids.to(device), mask.float().to(device)
+
+
 def encoder_outputs(batch: int, t5_lens, seed: int = 78, device="cpu"):
     """Synthetic encoder outputs for the sequence-generation models (SURVEY.md 8d): CLAP [B, 1, 512] L2-normalised (as
     the CLAP embedding is), Flan-T5 hidden states [B, L, 1024] N(0, 1) with L = max(t5_lens) and the padding mask of

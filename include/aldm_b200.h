@@ -28,6 +28,8 @@
  *   SequenceGenAudioMAECond.forward -> Sequence2AudioMAE.generate aldm_program_run(seqgen program: GPT-2 prefill +
  *       audiomae_gen/sequence_input.py:110-201,294-325,           7 KV-cached decode passes; ALDM_OP_SEQ_ASSEMBLE,
  *       encoders/modules.py:271-300                                ALDM_OP_KV_ATTN, ALDM_OP_SEQ_FEEDBACK)
+ *   FlanT5HiddenState.encode_text -> T5EncoderModel (from the      aldm_program_run(t5 program: embedding + 24
+ *       token ids)  encoders/modules.py:113-198                    blocks; ALDM_OP_T5_EMBED .. ALDM_OP_T5_GATE)
  *
  * Conventions
  *   - all pointers are DEVICE pointers unless named host_*; buffers are caller-owned (torch
@@ -51,7 +53,7 @@
 extern "C" {
 #endif
 
-#define ALDM_ABI_VERSION 9
+#define ALDM_ABI_VERSION 10
 #define ALDM_MAX_TAPS 16
 
 enum {
@@ -278,11 +280,62 @@ typedef struct aldm_seq_feedback_desc {
 } aldm_seq_feedback_desc;
 int aldm_seq_feedback(const aldm_seq_feedback_desc* d, void* stream);
 
+/* ---- Flan-T5 encoder from token ids (csrc/text/t5.cu) ----------------------------------------
+ * The residual stream is fp32 [B * L, C]; every projection is a two-plane GEMM.  Sequences hold at most 128 tokens (the
+ * tokenizer's max_length), heads of d_kv = 64. */
+
+/* out[r, :] = table[ids[r], :] (shared.weight, fp32, not scaled).  The host checks 0 <= id < vocab; an id outside that
+ * range writes a NaN row. */
+typedef struct aldm_t5_embed_desc {
+  const int64_t* ids;        /* [rows] */
+  const float* table;        /* [vocab, C] */
+  float* out;                /* [rows, C] */
+  int32_t rows, vocab, C;
+} aldm_t5_embed_desc;
+int aldm_t5_embed(const aldm_t5_embed_desc* d, void* stream);
+
+/* T5LayerNorm: y = gamma * (x * 1 / sqrt(mean(x^2) + eps)) per row of C (C % 128 == 0, <= 2048), fixed-order fp32 sum.
+ * Writes operand planes out_hi / out_lo [rows, ldo], or fp32 out_f32 [rows, ldo] when out_f32 is not NULL. */
+typedef struct aldm_t5_rmsnorm_desc {
+  const float* x;            /* [rows, C] */
+  const float* gamma;        /* [C] */
+  void* out_hi; void* out_lo;
+  float* out_f32;
+  int32_t rows, C, ldo;
+  float eps;
+} aldm_t5_rmsnorm_desc;
+int aldm_t5_rmsnorm(const aldm_t5_rmsnorm_desc* d, void* stream);
+
+/* Bidirectional self-attention of B sequences of L <= 128 tokens: s[i, j] = q_i . k_j (no 1/sqrt(d) scaling) +
+ * bias[h, j - i + 127]; keys with mask[b, j] != 1 get probability 0 (at least one key per row must be valid); fp32
+ * softmax and P V.  qkv [B * L, ld_qkv] holds q | k | v at columns [0, C), [C, 2C), [2C, 3C), head h at [h*64, +64).
+ * Output: planes [B * L, ldo].  d_kv != 64 is ALDM_E_UNSUPPORTED; L > 128 or heads * 64 != C is ALDM_E_SHAPE. */
+typedef struct aldm_t5_attn_desc {
+  const float* qkv;
+  const float* bias;         /* [heads, 255]: the relative-position bias for offsets j - i = -127 .. 127 */
+  const float* mask;         /* [B, L] */
+  void* out_hi; void* out_lo;
+  int32_t B, L, heads, d_kv, C, ld_qkv, ldo;
+} aldm_t5_attn_desc;
+int aldm_t5_attention(const aldm_t5_attn_desc* d, void* stream);
+
+/* Gated-GELU: y[r, c] = gelu_new(x[r, c]) * x[r, F + c] for c < F (x = the fp32 output of the fused [wi_0 | wi_1] GEMM),
+ * written as operand planes [rows, ldo].  Elements with |y| > 65504 or non-finite y, which the planes would clamp, are
+ * counted into *sat (atomically; the caller zeroes it and reads it back). */
+typedef struct aldm_t5_gate_desc {
+  const float* x;            /* [rows, ld_x] */
+  void* out_hi; void* out_lo;
+  uint32_t* sat;
+  int32_t rows, F, ld_x, ldo;
+} aldm_t5_gate_desc;
+int aldm_t5_gate(const aldm_t5_gate_desc* d, void* stream);
+
 /* ---- programs: flat op tables replayed on a stream / as a CUDA graph ---------------------- */
 
 enum { ALDM_OP_GEMM = 1, ALDM_OP_PREP = 2, ALDM_OP_ATTN = 3, ALDM_OP_SOFTMAX = 4, ALDM_OP_TEMB = 5,
        ALDM_OP_TRANSPOSE = 6, ALDM_OP_PACKB = 7, ALDM_OP_COPY = 8, ALDM_OP_SEQ_ASSEMBLE = 9, ALDM_OP_KV_ATTN = 10,
-       ALDM_OP_SEQ_FEEDBACK = 11 };
+       ALDM_OP_SEQ_FEEDBACK = 11, ALDM_OP_T5_EMBED = 12, ALDM_OP_T5_RMSNORM = 13, ALDM_OP_T5_ATTN = 14,
+       ALDM_OP_T5_GATE = 15 };
 
 typedef struct aldm_op {
   int32_t kind;
@@ -299,6 +352,10 @@ typedef struct aldm_op {
     aldm_seq_assemble_desc seq_assemble;
     aldm_kv_attn_desc kv_attn;
     aldm_seq_feedback_desc seq_feedback;
+    aldm_t5_embed_desc t5_embed;
+    aldm_t5_rmsnorm_desc t5_rmsnorm;
+    aldm_t5_attn_desc t5_attn;
+    aldm_t5_gate_desc t5_gate;
   } u;
 } aldm_op;
 
