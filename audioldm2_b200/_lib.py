@@ -17,7 +17,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libaldm_b200.so")
 SOURCES = ["gemm.cu", "prep.cu", "attention.cu", "elementwise.cu", "stft.cu", "program.cu", "engine_abi.cu", "microbench.cu",
-           "cond/seqgen.cu", "text/t5.cu"]
+           "cond/seqgen.cu", "text/t5.cu", "clap/clap_text.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
@@ -25,7 +25,7 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-
 NVCC = shutil.which("nvcc") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
 
 MAX_TAPS = 16
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 # enums (keep in sync with the header; checked by tests/test_abi.py against the header text)
 GEMM_TC, GEMM_SIMT, GEMM_TC_V1 = 0, 1, 2
@@ -40,6 +40,7 @@ PREP_COPY, PREP_SILU, PREP_LRELU, PREP_GN, PREP_GN_SILU, PREP_LN = 0, 1, 2, 3, 4
 OP_GEMM, OP_PREP, OP_ATTN, OP_SOFTMAX, OP_TEMB, OP_TRANSPOSE, OP_PACKB, OP_COPY = 1, 2, 3, 4, 5, 6, 7, 8
 OP_SEQ_ASSEMBLE, OP_KV_ATTN, OP_SEQ_FEEDBACK = 9, 10, 11
 OP_T5_EMBED, OP_T5_RMSNORM, OP_T5_ATTN, OP_T5_GATE = 12, 13, 14, 15
+OP_CLAP_EMBED, OP_CLAP_LN, OP_CLAP_ATTN, OP_CLAP_GELU, OP_CLAP_HEAD = 16, 17, 18, 19, 20
 
 
 class GemmDesc(C.Structure):
@@ -146,11 +147,42 @@ class T5GateDesc(C.Structure):
                 ("rows", C.c_int32), ("F", C.c_int32), ("ld_x", C.c_int32), ("ldo", C.c_int32)]
 
 
+class ClapEmbedDesc(C.Structure):
+    _fields_ = [("ids", C.c_void_p), ("word", C.c_void_p), ("pos", C.c_void_p), ("type", C.c_void_p), ("out", C.c_void_p),
+                ("B", C.c_int32), ("L", C.c_int32), ("vocab", C.c_int32), ("n_pos", C.c_int32), ("C", C.c_int32),
+                ("pad", C.c_int32)]
+
+
+class ClapLnDesc(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p), ("out_f32", C.c_void_p),
+                ("out_hi", C.c_void_p), ("out_lo", C.c_void_p), ("rows", C.c_int32), ("C", C.c_int32), ("ldo", C.c_int32),
+                ("eps", C.c_float)]
+
+
+class ClapAttnDesc(C.Structure):
+    _fields_ = [("qkv", C.c_void_p), ("mask", C.c_void_p), ("out_hi", C.c_void_p), ("out_lo", C.c_void_p),
+                ("B", C.c_int32), ("L", C.c_int32), ("heads", C.c_int32), ("C", C.c_int32), ("ld_qkv", C.c_int32),
+                ("ldo", C.c_int32)]
+
+
+class ClapGeluDesc(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("out_hi", C.c_void_p), ("out_lo", C.c_void_p),
+                ("rows", C.c_int32), ("F", C.c_int32), ("ld_x", C.c_int32), ("ldo", C.c_int32)]
+
+
+class ClapHeadDesc(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("wp_t", C.c_void_p), ("bp", C.c_void_p), ("w1_t", C.c_void_p), ("b1", C.c_void_p),
+                ("w2_t", C.c_void_p), ("b2", C.c_void_p), ("out", C.c_void_p),
+                ("B", C.c_int32), ("L", C.c_int32), ("C", C.c_int32), ("P", C.c_int32)]
+
+
 class _OpU(C.Union):
     _fields_ = [("gemm", GemmDesc), ("prep", PrepDesc), ("attn", AttnDesc), ("softmax", _Softmax),
                 ("temb", _Temb), ("transpose", _Transpose), ("packb", _PackB), ("copy", _Copy),
                 ("seq_assemble", SeqAssembleDesc), ("kv_attn", KvAttnDesc), ("seq_feedback", SeqFeedbackDesc),
-                ("t5_embed", T5EmbedDesc), ("t5_rmsnorm", T5RmsnormDesc), ("t5_attn", T5AttnDesc), ("t5_gate", T5GateDesc)]
+                ("t5_embed", T5EmbedDesc), ("t5_rmsnorm", T5RmsnormDesc), ("t5_attn", T5AttnDesc), ("t5_gate", T5GateDesc),
+                ("clap_embed", ClapEmbedDesc), ("clap_ln", ClapLnDesc), ("clap_attn", ClapAttnDesc), ("clap_gelu", ClapGeluDesc),
+                ("clap_head", ClapHeadDesc)]
 
 
 class Op(C.Structure):
@@ -234,6 +266,11 @@ def lib() -> C.CDLL:
         "aldm_t5_rmsnorm": (i32, [C.POINTER(T5RmsnormDesc), vp]),
         "aldm_t5_attention": (i32, [C.POINTER(T5AttnDesc), vp]),
         "aldm_t5_gate": (i32, [C.POINTER(T5GateDesc), vp]),
+        "aldm_clap_embed": (i32, [C.POINTER(ClapEmbedDesc), vp]),
+        "aldm_clap_layernorm": (i32, [C.POINTER(ClapLnDesc), vp]),
+        "aldm_clap_attention": (i32, [C.POINTER(ClapAttnDesc), vp]),
+        "aldm_clap_gelu": (i32, [C.POINTER(ClapGeluDesc), vp]),
+        "aldm_clap_head": (i32, [C.POINTER(ClapHeadDesc), vp]),
         "aldm_softmax_rows": (i32, [vp, i32, i32, f32, vp, vp, vp]),
         "aldm_timestep_embedding": (i32, [vp, i32, i32, vp, vp, vp, vp]),
         "aldm_ddim_step": (i32, [vp, vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, vp]),
@@ -285,6 +322,7 @@ def lib() -> C.CDLL:
 EXPORTED = ["aldm_gemm", "aldm_gemm_variant", "aldm_gemm_a_mode", "aldm_prep", "aldm_pack_b", "aldm_attention", "aldm_softmax_rows",
             "aldm_kv_attention", "aldm_seq_assemble", "aldm_seq_feedback",
             "aldm_t5_embed", "aldm_t5_rmsnorm", "aldm_t5_attention", "aldm_t5_gate",
+            "aldm_clap_embed", "aldm_clap_layernorm", "aldm_clap_attention", "aldm_clap_gelu", "aldm_clap_head",
             "aldm_timestep_embedding", "aldm_ddim_step", "aldm_masked_blend", "aldm_transpose_chw",
             "aldm_posterior_sample", "aldm_stft_mel", "aldm_program_create", "aldm_program_run",
             "aldm_program_run_range", "aldm_program_capture", "aldm_program_replay",

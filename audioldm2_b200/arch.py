@@ -427,3 +427,56 @@ def has_t5(cfg: dict) -> bool:
     """Configs whose UNet reads Flan-T5 states (a 1024-wide context): audioldm2-full / -large (next to the AudioMAE
     tokens) and the *_t5 models."""
     return 1024 in [c for c in (cfg["unet"].get("context_dim") or []) if c is not None]
+
+
+# --------------------------------------------------------------------------------------
+# CLAP text branch (CLAPAudioEmbeddingClassifierFreev2 with embed_mode "text", encoders/modules.py:546-745, and
+# CLAP.get_text_embedding, clap/open_clip/model.py:656-663, 730-750): HF RobertaModel(RobertaConfig("roberta-base")) --
+# 12 post-LN blocks, width 768, 12 heads of 64, erf-GELU feed-forward of 3072, LayerNorm eps 1e-5, learned positions
+# offset by the pad id -- then the tanh pooler on token 0, text_projection (Linear 768 -> 512, ReLU, Linear 512 -> 512)
+# and F.normalize.  The tokenizer (RobertaTokenizer, padding="max_length", max_length 512; "" -> [0, 2]) stays on the host.
+# --------------------------------------------------------------------------------------
+
+CLAP_TEXT = dict(d_model=768, n_head=12, d_head=64, d_ff=3072, n_layer=12, vocab=50265, max_positions=514, type_vocab=1,
+                 pad_id=1, bos_id=0, eos_id=2, eps=1e-5, joint_dim=512, max_len=512)
+
+
+def clap_text_param_shapes(n_layer: int = 12) -> Dict[str, Tuple[int, ...]]:
+    """name -> shape of the CLAP text branch's state dict (relative to the CLAP model, e.g. ``cond_stage_models.0.model.``):
+    HF ``RobertaModel`` keys under ``text_branch.`` and ``text_projection.{0,2}``."""
+    C, F, P = CLAP_TEXT["d_model"], CLAP_TEXT["d_ff"], CLAP_TEXT["joint_dim"]
+    e = "text_branch.embeddings"
+    S: Dict[str, Tuple[int, ...]] = {
+        f"{e}.word_embeddings.weight": (CLAP_TEXT["vocab"], C),
+        f"{e}.position_embeddings.weight": (CLAP_TEXT["max_positions"], C),
+        f"{e}.token_type_embeddings.weight": (CLAP_TEXT["type_vocab"], C),
+        f"{e}.LayerNorm.weight": (C,), f"{e}.LayerNorm.bias": (C,),
+    }
+    for i in range(n_layer):
+        b = f"text_branch.encoder.layer.{i}"
+        for n in ("query", "key", "value"):
+            S[f"{b}.attention.self.{n}.weight"] = (C, C)
+            S[f"{b}.attention.self.{n}.bias"] = (C,)
+        S[f"{b}.attention.output.dense.weight"] = (C, C)
+        S[f"{b}.attention.output.dense.bias"] = (C,)
+        S[f"{b}.attention.output.LayerNorm.weight"] = (C,)
+        S[f"{b}.attention.output.LayerNorm.bias"] = (C,)
+        S[f"{b}.intermediate.dense.weight"] = (F, C)
+        S[f"{b}.intermediate.dense.bias"] = (F,)
+        S[f"{b}.output.dense.weight"] = (C, F)
+        S[f"{b}.output.dense.bias"] = (C,)
+        S[f"{b}.output.LayerNorm.weight"] = (C,)
+        S[f"{b}.output.LayerNorm.bias"] = (C,)
+    S["text_branch.pooler.dense.weight"] = (C, C)
+    S["text_branch.pooler.dense.bias"] = (C,)
+    S["text_projection.0.weight"] = (P, C)
+    S["text_projection.0.bias"] = (P,)
+    S["text_projection.2.weight"] = (P, P)
+    S["text_projection.2.bias"] = (P,)
+    return S
+
+
+def has_clap(cfg: dict) -> bool:
+    """Configs conditioned on the CLAP text embedding: audioldm2-full / -large (GPT-2's first input) and audioldm_48k (the
+    FiLM vector, 512 wide).  The tiny FiLM test configs (dim 24) are not."""
+    return has_seqgen(cfg) or cfg["unet"].get("extra_film_condition_dim") == CLAP_TEXT["joint_dim"]

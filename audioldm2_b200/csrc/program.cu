@@ -51,6 +51,11 @@ int t5_embed_launch(const aldm_t5_embed_desc& d, cudaStream_t st);
 int t5_rmsnorm_launch(const aldm_t5_rmsnorm_desc& d, cudaStream_t st);
 int t5_attention_launch(const aldm_t5_attn_desc& d, cudaStream_t st);
 int t5_gate_launch(const aldm_t5_gate_desc& d, cudaStream_t st);
+int clap_embed_launch(const aldm_clap_embed_desc& d, cudaStream_t st);
+int clap_layernorm_launch(const aldm_clap_ln_desc& d, cudaStream_t st);
+int clap_attention_launch(const aldm_clap_attn_desc& d, cudaStream_t st);
+int clap_gelu_launch(const aldm_clap_gelu_desc& d, cudaStream_t st);
+int clap_head_launch(const aldm_clap_head_desc& d, cudaStream_t st);
 
 }  // namespace aldm
 
@@ -86,6 +91,11 @@ static int run_op(const aldm_op& op, cudaStream_t st) {
     case ALDM_OP_T5_RMSNORM: return t5_rmsnorm_launch(op.u.t5_rmsnorm, st);
     case ALDM_OP_T5_ATTN: return t5_attention_launch(op.u.t5_attn, st);
     case ALDM_OP_T5_GATE: return t5_gate_launch(op.u.t5_gate, st);
+    case ALDM_OP_CLAP_EMBED: return clap_embed_launch(op.u.clap_embed, st);
+    case ALDM_OP_CLAP_LN: return clap_layernorm_launch(op.u.clap_ln, st);
+    case ALDM_OP_CLAP_ATTN: return clap_attention_launch(op.u.clap_attn, st);
+    case ALDM_OP_CLAP_GELU: return clap_gelu_launch(op.u.clap_gelu, st);
+    case ALDM_OP_CLAP_HEAD: return clap_head_launch(op.u.clap_head, st);
     case ALDM_OP_COPY:
       ALDM_CHECK_CUDA(cudaMemcpyAsync(op.u.copy.dst, op.u.copy.src, (size_t)op.u.copy.bytes, cudaMemcpyDeviceToDevice, st));
       return ALDM_OK;

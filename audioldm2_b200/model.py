@@ -82,6 +82,26 @@ def split_t5_state_dict(state_dict: Dict[str, torch.Tensor], prefix: str) -> Dic
     return out
 
 
+def split_clap_text_state_dict(state_dict: Dict[str, torch.Tensor], prefix: str) -> Dict[str, torch.Tensor]:
+    """The CLAP text branch's weights from a reference checkpoint: the keys under ``prefix`` (the CLAP model, e.g.
+    ``cond_stage_models.0.model.``), named and shaped as arch.clap_text_param_shapes.  The ``embeddings.position_ids`` /
+    ``token_type_ids`` buffers that older transformers saved and everything of the audio branch are ignored.  Raises
+    KeyError for a missing key, ValueError for a wrong shape."""
+    tail = ".attention.output.LayerNorm.weight"
+    n_layer = len([k for k in state_dict if k.startswith(prefix + "text_branch.encoder.layer.") and k.endswith(tail)])
+    if n_layer == 0:
+        raise KeyError(f"checkpoint has no RoBERTa layers under {prefix}text_branch.encoder.layer.")
+    out = {}
+    for k, shp in arch.clap_text_param_shapes(n_layer).items():
+        v = state_dict.get(prefix + k)
+        if v is None:
+            raise KeyError(f"checkpoint has no {prefix + k} (needed by the CLAP text encoder)")
+        if tuple(v.shape) != tuple(shp):
+            raise ValueError(f"{prefix + k}: shape {tuple(v.shape)}, expected {shp}")
+        out[k] = v
+    return out
+
+
 def reorder_cond_dict(cond_dict: dict, conditioning_key: Sequence[str]) -> dict:
     """LatentDiffusion.reorder_cond_dict (ddpm.py:1028-1032): the UNet consumes the conditions in the order of
     ``conditioning_key`` (the config's list), not in the dict's insertion order."""

@@ -15,6 +15,10 @@ network.  What differs, by design of this tier:
   reference's own key, ``crossattn_flan_t5`` = [input_ids (integer) [B, L], attention_mask [B, L]] (plus
   ``film_clap_cond1`` for the sequence-generation models): the T5 states are then encoded natively
   (t5.NativeFlanT5Encoder) before anything else, in the conditional and the unconditional dict alike;
+  and for every model conditioned on the CLAP text embedding (audioldm2-full / -large, audioldm_48k), the RoBERTa
+  tokenizer's output under the reference's key, ``film_clap_cond1`` = [input_ids (integer) [B, L], attention_mask [B, L]]:
+  the embedding is then computed natively (clap.NativeCLAPTextEncoder) before everything else, with the reference's random
+  replacement of prompt rows by CLAP("") (clap_replacement_draws);
 * candidate re-ranking (ddpm.py:1554-1568) uses ``latent_diffusion.ranker(waveform [n,1,L], texts) -> similarity [n]``
   (the reference's ``clap.cos_similarity``); without one the first candidate of each prompt is returned and a
   warning says so;
@@ -105,6 +109,77 @@ class SyntheticTokenIds:
         return out
 
 
+class SyntheticPromptTokens:
+    """Seeded tokenizer output for every model conditioned on the CLAP text embedding (opt-in): ``film_clap_cond1`` =
+    [ids, mask] padded to the RoBERTa tokenizer's 512 (padding="max_length"; row i holds ``lens[i % len]`` tokens, BOS and
+    EOS included), plus Flan-T5 ids (SyntheticTokenIds' layout, ``t5_lens``) where the model has a Flan-T5 context.  The
+    unconditional branch is the reference's: the tokenization of "" on every row for audioldm_48k, zero AudioMAE tokens
+    and T5("") for the sequence-generation models."""
+
+    def __init__(self, cfg: dict, seed: int = 81, lens=(24, 11, 5), t5_lens=(32, 19, 7), device="cpu"):
+        if not arch.has_clap(cfg):
+            raise ValueError(f"{cfg.get('name')}: CLAP token ids need a model conditioned on the CLAP text embedding")
+        self.cfg, self.seed, self.lens, self.device = cfg, seed, tuple(lens), device
+        self._t5 = SyntheticTokenIds(cfg, seed=seed + 1, lens=t5_lens, device=device) if arch.has_t5(cfg) else None
+
+    def cond(self, batch: dict) -> dict:
+        n = len(batch["text"])
+        ids, mask = synth.clap_token_ids([self.lens[i % len(self.lens)] for i in range(n)], seed=self.seed, device=self.device)
+        out = {"film_clap_cond1": [ids, mask]}
+        if self._t5 is not None:
+            out["crossattn_flan_t5"] = self._t5.cond(batch)["crossattn_flan_t5"]
+        return out
+
+    def uncond(self, n: int) -> dict:
+        if self._t5 is not None:                    # SequenceGenAudioMAECond's cfg_uncond and T5(""): no CLAP entry
+            return self._t5.uncond(n)
+        from .clap import empty_prompt
+        return {"film_clap_cond1": list(empty_prompt(n, device=self.device))}
+
+
+def is_clap_token_level(cond) -> bool:
+    """The CLAP entry holds the tokenizer's output (integer ids) rather than the embedding."""
+    if not isinstance(cond, dict) or not isinstance(cond.get("film_clap_cond1"), (list, tuple)):
+        return False
+    ids = cond["film_clap_cond1"][0]
+    return torch.is_tensor(ids) and not ids.dtype.is_floating_point and not ids.dtype.is_complex
+
+
+def clap_replacement_draws(n: int, extra: bool) -> list:
+    """The CPU draws of the reference's get_input for the CLAP conditioner, in its order: with ``extra`` (every call of a
+    model after its first: conditional_dry_run_finished) LatentDiffusion.make_decision(0.0) draws one torch.rand(1)
+    (ddpm.py:852-854); then CLAPAudioEmbeddingClassifierFreev2.forward draws one per prompt row, in row order, and replaces
+    the row by CLAP("") below unconditional_prob = 0.1 (encoders/modules.py:731-733).  -> the n decisions."""
+    if extra:
+        torch.rand(1)                               # make_decision(0.0): drawn, never true
+    return [float(torch.rand(1)) < 0.1 for _ in range(n)]
+
+
+def encode_clap_tokens(cfg: dict, cond: dict, encoder: Callable[[], object], unconditional: bool = False,
+                       decide: Optional[Callable[[int], list]] = None) -> dict:
+    """Replace token-level ``film_clap_cond1`` = [ids, mask] by the embedding [B, 1, 512] (every other entry is kept, in
+    order); anything else is returned as it is, the encoder is never built and nothing is drawn.  In the conditional dict
+    ``decide(B)`` gives the rows replaced by CLAP("") (clap_replacement_draws; None: no replacement).  In the
+    unconditional dict, rows that are all the tokenization of "" go through ``encoder().unconditional()``, computed once
+    and cached like the reference's unconditional_token (get_unconditional_condition, encoders/modules.py:606-610)."""
+    if not is_clap_token_level(cond):
+        return cond
+    if not arch.has_clap(cfg):
+        raise ValueError(f"{cfg.get('name')} has no CLAP text conditioning: token ids under film_clap_cond1 do not apply")
+    from .clap import is_empty_prompt
+    ids, mask = cond["film_clap_cond1"]
+    enc = encoder()
+    if unconditional and is_empty_prompt(ids, mask):
+        e = enc.unconditional().expand(ids.shape[0], -1).clone()
+    else:
+        e = enc.embed(ids, mask)
+        if not unconditional and decide is not None:
+            rows = [i for i, r in enumerate(decide(ids.shape[0])) if r]
+            if rows:
+                e[rows] = enc.unconditional().to(e.device)
+    return {k: (e[:, None, :] if k == "film_clap_cond1" else v) for k, v in cond.items()}
+
+
 def is_token_level(cond) -> bool:
     """The Flan-T5 entry holds the tokenizer's output (integer ids) rather than hidden states."""
     if not isinstance(cond, dict) or not isinstance(cond.get("crossattn_flan_t5"), (list, tuple)):
@@ -182,9 +257,10 @@ class NativeAudioLDM2:
 
     def __init__(self, cfg: dict, unet_sd, vae_sd, vocoder_sd, device, scale_factor: float = 1.0, ctx_max_len=None,
                  cond_provider=None, ranker: Optional[Callable] = None, seqgen_sd=None, t5_sd=None, t5_uncond_sd=None,
-                 **engine_kw):
+                 clap_sd=None, **engine_kw):
         """``t5_sd`` / ``t5_uncond_sd``: the Flan-T5 weights of the conditional and of the unconditional branch (or callables
-        that return them, for weights made on first use); ``t5_uncond_sd`` None means the same weights."""
+        that return them, for weights made on first use); ``t5_uncond_sd`` None means the same weights.  ``clap_sd``: the
+        CLAP text branch's weights (or a callable)."""
         self.cfg, self.device = cfg, torch.device(device)
         self._sd = (unet_sd, vae_sd, vocoder_sd)
         self.scale_factor = scale_factor
@@ -199,6 +275,9 @@ class NativeAudioLDM2:
         self._seqgen = None
         self._t5_sd, self._t5_uncond_sd = t5_sd, t5_uncond_sd
         self._t5 = None
+        self._clap_sd = clap_sd
+        self._clap = None
+        self.conditional_dry_run_finished = False           # LatentDiffusion's flag (ddpm.py:852-854, 916-917)
 
     # ---- AudioMAE token generator (built on first use: UNet-boundary providers never pay for it) ----------------------
     def seqgen(self):
@@ -230,15 +309,35 @@ class NativeAudioLDM2:
             self._t5 = (enc_c, enc_u)
         return self._t5
 
+    # ---- CLAP text encoder (built on first token-level use) ------------------------------------------------
+    def clap_encoder(self):
+        if self._clap is None:
+            if self._clap_sd is None:
+                raise ValueError("token-level film_clap_cond1 needs the CLAP text weights, which this model was built without")
+            from .clap import NativeCLAPTextEncoder
+            self._clap = NativeCLAPTextEncoder(self._clap_sd() if callable(self._clap_sd) else self._clap_sd, self.device)
+        return self._clap
+
     def conditioning(self, batch) -> dict:
-        """The provider's conditioning of the call's B prompts: token ids encoded by Flan-T5, then the AudioMAE tokens
-        generated when it holds encoder outputs."""
-        cond = encode_tokens(self.cfg, self.cond_provider.cond(batch), lambda: self.t5_encoders()[0])
+        """The provider's conditioning of the call's B prompts, as the reference's get_input makes it (after the posterior
+        draw): CLAP token ids embedded, with the reference's random replacement by CLAP(""), and Flan-T5 token ids
+        encoded; then the AudioMAE tokens generated when it holds encoder outputs."""
+        extra = self.conditional_dry_run_finished
+        self.conditional_dry_run_finished = True
+        cond = encode_clap_tokens(self.cfg, self.cond_provider.cond(batch), self.clap_encoder,
+                                  decide=lambda n: clap_replacement_draws(n, extra))
+        cond = encode_tokens(self.cfg, cond, lambda: self.t5_encoders()[0])
         return route_conditioning(self.cfg, cond, self.seqgen)
 
+    def _sharded_conditioning(self, batch, lo: int, hi: int) -> dict:
+        """Rows [lo, hi) of the conditioning of the whole call: every rank makes the draws of all B prompts, so the
+        replacement decisions and the CPU generator state are those of one process."""
+        return parallel.shard_rows(self.conditioning(batch), lo, hi)
+
     def unconditioning(self, n: int, uncond=None) -> dict:
-        """The unconditional branch (the provider's unless given), with token ids encoded by the unconditional encoder."""
+        """The unconditional branch (the provider's unless given), with token ids encoded by the unconditional encoders."""
         u = self.cond_provider.uncond(n) if uncond is None else uncond
+        u = encode_clap_tokens(self.cfg, u, self.clap_encoder, unconditional=True)
         return encode_tokens(self.cfg, u, lambda: self.t5_encoders()[1], unconditional=True)
 
     # ---- engines -------------------------------------------------------------------------------------
@@ -303,7 +402,8 @@ class NativeAudioLDM2:
         B = len(batch["text"])
         local = {k: (v[lo:hi] if (torch.is_tensor(v) or isinstance(v, list)) and len(v) == B else v) for k, v in batch.items()}
         rows = [i + k * B for k in range(n_gen) for i in range(lo, hi)]
-        cond_l = parallel.shard_rows(self.conditioning(batch), lo, hi)             # conditioning of the whole call, this rank's rows
+        # conditioning of the whole call, this rank's rows: made by _generate_local after the posterior draw, as in one process
+        cond_l = lambda: self._sharded_conditioning(batch, lo, hi)
         out = self._generate_local(local, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, (B, rows), cond_l)
         full = parallel.all_gather_rows(torch.from_numpy(out).to(self.device), B)
         return self._egress(full)
@@ -336,7 +436,7 @@ class NativeAudioLDM2:
             mask[:, int(T * tmask[0]):int(T * tmask[1]), :] = 0
             mask[:, :, int(F_ * fmask[0]):int(F_ * fmask[1])] = 0
             mask = mask[:, None].contiguous()
-        cond = _tile(cond_rows if cond_rows is not None else self.conditioning(batch), n_gen)
+        cond = _tile(cond_rows() if cond_rows is not None else self.conditioning(batch), n_gen)
         if guidance != 1.0:
             uncond = self.unconditioning(Bl, uncond)                                      # ddpm.py:1529-1536
         texts = list(batch["text"]) * n_gen
@@ -365,7 +465,9 @@ def build_model(ckpt_path=None, config=None, device=None, model_name="audioldm2-
     generator's inner T5 (``cond_stage_models.<seqgen_index>.cond_stage_models.<t5_index>.model.``, t5_index 1 by default:
     get_input skips a key an earlier model already produced, ddpm.py:861-862) and T5("") with the top-level copy
     (``cond_stage_models.<t5_index>.model.``, ddpm.py:1529-1533); the *_t5 models use ``cond_stage_models.<t5_index>``
-    (default 0) for both.  Synthetic weights are generated on first token-level use."""
+    (default 0) for both.  The CLAP text weights, for token-level ``film_clap_cond1``: the generator's first inner model
+    (``cond_stage_models.<seqgen_index>.cond_stage_models.0.model.``) for audioldm2-full / -large,
+    ``cond_stage_models.0.model.`` for audioldm_48k.  Synthetic weights are generated on first token-level use."""
     if device is None or device == "auto":
         device = torch.device("cuda:0")          # the native path has no CPU / MPS fallback
     cfg = arch.model_config(model_name) if config is None else config
@@ -380,6 +482,7 @@ def build_model(ckpt_path=None, config=None, device=None, model_name="audioldm2-
         seq = synth.seqgen_state_dict() if arch.has_seqgen(cfg) else None
         t5c = synth.t5_state_dict if arch.has_t5(cfg) else None
         t5u = None
+        clap = synth.clap_text_state_dict if arch.has_clap(cfg) else None
         if ctx_max_len is None:
             n_cross = len([c for c in cfg["unet"]["context_dim"] if c is not None])
             ctx_max_len = (8, t5_len) if n_cross > 1 else (t5_len,)
@@ -394,8 +497,13 @@ def build_model(ckpt_path=None, config=None, device=None, model_name="audioldm2-
             t5u = model.split_t5_state_dict(sd, f"cond_stage_models.{j}.model.")
         elif arch.has_t5(cfg):
             t5c = model.split_t5_state_dict(sd, f"cond_stage_models.{t5_index or 0}.model.")
+        clap = None
+        if arch.has_seqgen(cfg):
+            clap = model.split_clap_text_state_dict(sd, f"cond_stage_models.{seqgen_index}.cond_stage_models.0.model.")
+        elif arch.has_clap(cfg):
+            clap = model.split_clap_text_state_dict(sd, "cond_stage_models.0.model.")
     ld = NativeAudioLDM2(cfg, un, vae, voc, device, scale_factor=sf, ctx_max_len=ctx_max_len, seqgen_sd=seq,
-                         t5_sd=t5c, t5_uncond_sd=t5u,
+                         t5_sd=t5c, t5_uncond_sd=t5u, clap_sd=clap,
                          cond_provider=cond_provider or SyntheticConditioning(cfg, t5_len=t5_len, device=device), ranker=ranker,
                          **engine_kw)
     ld.model_name = model_name

@@ -263,6 +263,39 @@ class Plan:
                 for name in ("x", "out_hi", "out_lo", "sat"):
                     setattr(a, name, P(o.get(name)))
                 a.rows, a.F, a.ld_x, a.ldo = int(o["rows"]), int(o["F"]), int(o["ld_x"]), int(o["ldo"])
+            elif k == "clap_embed":
+                op.kind = _lib.OP_CLAP_EMBED
+                a = op.u.clap_embed
+                for name in ("ids", "word", "pos", "type", "out"):
+                    setattr(a, name, P(o[name]))
+                for name in ("B", "L", "vocab", "n_pos", "C", "pad"):
+                    setattr(a, name, int(o[name]))
+            elif k == "clap_ln":
+                op.kind = _lib.OP_CLAP_LN
+                a = op.u.clap_ln
+                for name in ("x", "gamma", "beta", "out_f32", "out_hi", "out_lo"):
+                    setattr(a, name, P(o.get(name)))
+                a.rows, a.C, a.ldo, a.eps = int(o["rows"]), int(o["C"]), int(o["ldo"]), float(o["eps"])
+            elif k == "clap_attn":
+                op.kind = _lib.OP_CLAP_ATTN
+                a = op.u.clap_attn
+                for name in ("qkv", "mask", "out_hi", "out_lo"):
+                    setattr(a, name, P(o.get(name)))
+                for name in ("B", "L", "heads", "C", "ld_qkv", "ldo"):
+                    setattr(a, name, int(o[name]))
+            elif k == "clap_gelu":
+                op.kind = _lib.OP_CLAP_GELU
+                a = op.u.clap_gelu
+                for name in ("x", "out_hi", "out_lo"):
+                    setattr(a, name, P(o.get(name)))
+                a.rows, a.F, a.ld_x, a.ldo = int(o["rows"]), int(o["F"]), int(o["ld_x"]), int(o["ldo"])
+            elif k == "clap_head":
+                op.kind = _lib.OP_CLAP_HEAD
+                a = op.u.clap_head
+                for name in ("x", "wp_t", "bp", "w1_t", "b1", "w2_t", "b2", "out"):
+                    setattr(a, name, P(o[name]))
+                for name in ("B", "L", "C", "P"):
+                    setattr(a, name, int(o[name]))
             elif k == "copy":
                 op.kind = _lib.OP_COPY
                 c = op.u.copy
@@ -1234,6 +1267,176 @@ def build_t5(sd: Optional[Dict[str, torch.Tensor]], batch: int, length: int, wei
     P.ops.append(dict(kind="t5_rmsnorm", tag=P.tag, x=x.ref, gamma=r["final"], out_hi=None, out_lo=None, out_f32=hidden,
                       rows=R, C=C, ldo=C, eps=eps))
     P.free(x)
+    P.mark("end")
+    assert P.arena.size == 0, "encoder plans reference the shared weight arena only"
+    pl = P.finish(io, meta=dict(B=B, L=L, n_layer=W.n_layer))
+    pl.arena = W.arena
+    return pl
+
+
+# ==============================================================================================
+# CLAP text embedding from token ids (CLAP.get_text_embedding, clap/open_clip/model.py:656-663, 730-750; HF RobertaModel)
+# ==============================================================================================
+CLAP_BN = 64         # N tile of every encoder GEMM: the same packed weights serve plans of 2 to 4096 rows
+FP16_MAX = 65504.0
+
+
+@dataclass
+class ClapWeights:
+    """The text branch's weight arena, packed once and shared by the plans of every (batch, length); ``bounds``: name ->
+    the largest magnitude a value entering that operand plane can take (pack_clap_weights)."""
+    arena: torch.Tensor
+    n_layer: int
+    refs: Dict[str, object]
+    bounds: Dict[str, float]
+
+
+def clap_plane_bounds(sd: Dict[str, torch.Tensor], n_layer: int) -> Dict[str, float]:
+    """Bounds, from the weights alone, on every value the encoder writes into fp16 operand planes.  RoBERTa is post-LN, so
+    each such value is a LayerNorm output y = gamma * z + beta with ||z||_2 <= sqrt(C) (z has zero mean and unit variance
+    up to eps), a linear function of one, or a convex combination / GELU of those:
+      LayerNorm output            |y_c| <= |gamma_c| sqrt(C) + |beta_c|
+      u = W y + b (v, and the     |u_n| <= ||w_n * gamma||_2 sqrt(C) + |w_n . beta| + |b_n|  (Cauchy-Schwarz)
+      intermediate pre-activation)
+      attention output            a mix of rows of v with weights summing to 1: bounded by v's bound
+      GELU output                 |gelu(u)| <= |u|
+    name (the HF module) -> bound, in float64."""
+    C = arch.CLAP_TEXT["d_model"]
+    rc = math.sqrt(C)
+    d = lambda n: sd[n].double()
+
+    def ln(n):
+        return float((d(n + ".weight").abs() * rc + d(n + ".bias").abs()).max())
+
+    def lin(n, ln_name):
+        w, b = d(n + ".weight"), d(n + ".bias")
+        g, be = d(ln_name + ".weight"), d(ln_name + ".bias")
+        return float(((w * g[None]).norm(dim=1) * rc + (w @ be).abs() + b.abs()).max())
+
+    prev = "text_branch.embeddings.LayerNorm"
+    out = {prev: ln(prev)}
+    for i in range(n_layer):
+        b = f"text_branch.encoder.layer.{i}"
+        out[f"{b}.attention.self.value"] = lin(f"{b}.attention.self.value", prev)
+        out[f"{b}.attention.output.LayerNorm"] = ln(f"{b}.attention.output.LayerNorm")
+        out[f"{b}.intermediate.dense"] = lin(f"{b}.intermediate.dense", f"{b}.attention.output.LayerNorm")
+        prev = f"{b}.output.LayerNorm"
+        out[prev] = ln(prev)
+    return out
+
+
+def pack_clap_weights(sd: Dict[str, torch.Tensor], **pk) -> ClapWeights:
+    """Weights of split_clap_text_state_dict / synth.clap_text_state_dict -> arena: the word, position and token-type
+    embeddings in fp32 (the embedding gather), LayerNorm vectors, per block the fused [query | key | value], attention
+    output, intermediate and output matrices (with biases) as two-plane tile images, and the pooler / projection in fp32,
+    transposed ([in, out]) for the head kernel.  Raises ValueError, naming the layer, if a value entering an operand plane
+    could exceed the fp16 range (clap_plane_bounds): the planes would clamp it, so such weights are refused here rather
+    than counted at run time."""
+    n_layer = len([k for k in sd if k.startswith("text_branch.encoder.layer.") and k.endswith(".attention.output.LayerNorm.weight")])
+    if n_layer == 0:
+        raise KeyError("state dict holds no RoBERTa layers (text_branch.encoder.layer.<i>.*)")
+    bounds = clap_plane_bounds(sd, n_layer)
+    for name, v in bounds.items():
+        if not v <= FP16_MAX:
+            raise ValueError(f"CLAP text branch: values entering the fp16 operand planes after {name} can reach {v:.6g}, "
+                             f"beyond the fp16 range ({FP16_MAX:g}); these weights cannot be encoded without clamping")
+    P = Planner(**pk)
+
+    def lin(names) -> WMat:
+        w = torch.cat([sd[n + ".weight"].float() for n in names], 0)
+        wm, taps, cp = packing.conv_weight_matrix(w)
+        return P.wmat(wm, torch.cat([sd[n + ".bias"].float() for n in names], 0), taps, cp, bn=CLAP_BN)
+
+    e = "text_branch.embeddings"
+    vec2 = lambda n: (P.vec(sd[n + ".weight"]), P.vec(sd[n + ".bias"]))
+    r: Dict[str, object] = {
+        "word": P.vec(sd[f"{e}.word_embeddings.weight"]),
+        "pos": P.vec(sd[f"{e}.position_embeddings.weight"]),
+        "type": P.vec(sd[f"{e}.token_type_embeddings.weight"][0]),
+        "ln_emb": vec2(f"{e}.LayerNorm"),
+        "wp_t": P.vec(sd["text_branch.pooler.dense.weight"].float().t()), "bp": P.vec(sd["text_branch.pooler.dense.bias"]),
+        "w1_t": P.vec(sd["text_projection.0.weight"].float().t()), "b1": P.vec(sd["text_projection.0.bias"]),
+        "w2_t": P.vec(sd["text_projection.2.weight"].float().t()), "b2": P.vec(sd["text_projection.2.bias"]),
+    }
+    for i in range(n_layer):
+        b = f"text_branch.encoder.layer.{i}"
+        r[f"{i}.qkv"] = lin([f"{b}.attention.self.{n}" for n in ("query", "key", "value")])
+        r[f"{i}.o"] = lin([f"{b}.attention.output.dense"])
+        r[f"{i}.ln1"] = vec2(f"{b}.attention.output.LayerNorm")
+        r[f"{i}.inter"] = lin([f"{b}.intermediate.dense"])
+        r[f"{i}.out"] = lin([f"{b}.output.dense"])
+        r[f"{i}.ln2"] = vec2(f"{b}.output.LayerNorm")
+    return ClapWeights(P.arena.build(), n_layer, r, bounds)
+
+
+def build_clap_text(sd: Optional[Dict[str, torch.Tensor]], batch: int, length: int, weights: Optional[ClapWeights] = None,
+                    **pk) -> Plan:
+    """CLAP.get_text_embedding(input_ids, attention_mask) for one (batch B, length L <= 512), in fp32.  The caller plans on
+    the longest valid row (clap.effective_length), not on the tokenizer's 512: the embedding reads token 0 of the last
+    layer only, and padded keys have probability 0 in every layer.
+
+    io: ids [B, L] int64, mask [B, L] fp32 (1 = token) in; embed [B, 512] fp32 out.  Launches: the embedding, its
+    LayerNorm, 8 per block (QKV GEMM, attention, attention-output GEMM + residual, LayerNorm, intermediate GEMM, GELU,
+    output GEMM + residual, LayerNorm) and the head.  Marks "begin", "end".  The plan references the arena of
+    ``weights`` (packed from ``sd`` when None)."""
+    W = weights if weights is not None else pack_clap_weights(sd, **pk)
+    P = Planner(**pk)
+    B, L = int(batch), int(length)
+    if B < 1 or not 1 <= L <= arch.CLAP_TEXT["max_len"]:
+        raise ValueError(f"clap: batch {B}, length {L} (1 .. {arch.CLAP_TEXT['max_len']} tokens)")
+    A = arch.CLAP_TEXT
+    C, H, Fd, Pj, eps = A["d_model"], A["n_head"], A["d_ff"], A["joint_dim"], A["eps"]
+    R = B * L
+    r = W.refs
+    ids = P.raw(R * 8)
+    mask = P.raw(R * 4)
+    embed = P.raw(B * Pj * 4)
+    io = dict(ids=("i64", ids, (B, L)), mask=("f32", mask, (B, L)), embed=("f32", embed, (B, Pj)))
+
+    def layernorm(src: F32, g) -> Tuple[F32, Planes]:
+        y, a = P.f32(R, C), P.planes(R, C)
+        P.ops.append(dict(kind="clap_ln", tag=P.tag, x=src.ref, gamma=g[0], beta=g[1], out_f32=y.ref, out_hi=a.hi, out_lo=a.lo,
+                          rows=R, C=C, ldo=a.Cp, eps=eps))
+        return y, a
+
+    P.mark("begin")
+    P.tag = 0
+    x0 = P.f32(R, C)
+    P.ops.append(dict(kind="clap_embed", tag=0, ids=ids, word=r["word"], pos=r["pos"], type=r["type"], out=x0.ref, B=B, L=L,
+                      vocab=A["vocab"], n_pos=A["max_positions"], C=C, pad=A["pad_id"]))
+    x, a = layernorm(x0, r["ln_emb"])
+    P.free(x0)
+    for i in range(W.n_layer):
+        P.tag = 1 + i
+        # RobertaAttention: x = LN(x + dense(attn(x)))
+        qkv = P.f32(R, 3 * C)
+        P.gemm(a, r[f"{i}.qkv"], B=1, H=R, out=qkv)
+        P.free(a)
+        o = P.planes(R, C)
+        P.ops.append(dict(kind="clap_attn", tag=P.tag, qkv=qkv.ref, mask=mask, out_hi=o.hi, out_lo=o.lo, B=B, L=L, heads=H, C=C,
+                          ld_qkv=3 * C, ldo=o.Cp))
+        P.free(qkv)
+        y = P.f32(R, C)
+        P.gemm(o, r[f"{i}.o"], B=1, H=R, out=y, res=x)
+        P.free(o, x)
+        x2, a2 = layernorm(y, r[f"{i}.ln1"])
+        P.free(y)
+        # RobertaIntermediate + RobertaOutput: x = LN(x + dense(gelu(dense(x))))
+        hm = P.f32(R, Fd)
+        P.gemm(a2, r[f"{i}.inter"], B=1, H=R, out=hm)
+        P.free(a2)
+        g = P.planes(R, Fd)
+        P.ops.append(dict(kind="clap_gelu", tag=P.tag, x=hm.ref, out_hi=g.hi, out_lo=g.lo, rows=R, F=Fd, ld_x=Fd, ldo=g.Cp))
+        P.free(hm)
+        y = P.f32(R, C)
+        P.gemm(g, r[f"{i}.out"], B=1, H=R, out=y, res=x2)
+        P.free(g, x2)
+        x, a = layernorm(y, r[f"{i}.ln2"])
+        P.free(y)
+    P.tag = 1 + W.n_layer
+    P.ops.append(dict(kind="clap_head", tag=P.tag, x=x.ref, wp_t=r["wp_t"], bp=r["bp"], w1_t=r["w1_t"], b1=r["b1"],
+                      w2_t=r["w2_t"], b2=r["b2"], out=embed, B=B, L=L, C=C, P=Pj))
+    P.free(x, a)
     P.mark("end")
     assert P.arena.size == 0, "encoder plans reference the shared weight arena only"
     pl = P.finish(io, meta=dict(B=B, L=L, n_layer=W.n_layer))

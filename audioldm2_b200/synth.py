@@ -141,6 +141,46 @@ def token_ids(lens, seed: int = 79, device="cpu"):
     return ids.to(device), mask.float().to(device)
 
 
+def clap_text_state_dict(seed: int = 1239, n_layer: int = 12) -> Dict[str, torch.Tensor]:
+    """Seeded CLAP text branch (HF ``RobertaModel`` keys under ``text_branch.`` plus ``text_projection``,
+    arch.clap_text_param_shapes).  Not ``_fill``: every matrix is N(0, 1 / fan_in), so that each projection of a LayerNorm
+    output is O(1) -- logits q.k / 8 of a few units, pooler pre-activations O(1) so that tanh is exercised on its
+    nonlinear part; biases and LayerNorm offsets 0.1 N(0, 1), LayerNorm weights 1 + 0.1 N(0, 1), embeddings N(0, 1)."""
+    shapes = arch.clap_text_param_shapes(n_layer)
+    g = torch.Generator(device="cpu")
+    g.manual_seed(seed)
+    out = {}
+    for name in sorted(shapes):
+        shp = shapes[name]
+        t = torch.randn(shp, generator=g)
+        if "embeddings." in name and len(shp) == 2:
+            pass
+        elif name.endswith("LayerNorm.weight"):
+            t = 1.0 + 0.1 * t
+        elif len(shp) == 1:
+            t = 0.1 * t
+        else:
+            t = t / math.sqrt(shp[1])
+        out[name] = t.contiguous()
+    return out
+
+
+def clap_token_ids(lens, L: int = 512, seed: int = 80, device="cpu"):
+    """Seeded RoBERTa tokenizer output as the reference pads it (padding="max_length"): ids [B, L] int64 and
+    attention_mask [B, L] float.  Row i holds lens[i] tokens -- BOS (0), lens[i] - 2 ids drawn from [3, vocab), EOS (2) --
+    then pad (1)."""
+    g = torch.Generator(device="cpu"); g.manual_seed(seed)
+    lens = [int(n) for n in lens]
+    assert min(lens) >= 2 and max(lens) <= L <= arch.CLAP_TEXT["max_len"]
+    ids = torch.randint(3, arch.CLAP_TEXT["vocab"], (len(lens), L), generator=g)
+    n = torch.tensor(lens)[:, None]
+    pos = torch.arange(L)[None, :]
+    ids[:, 0] = arch.CLAP_TEXT["bos_id"]
+    ids = torch.where(pos == n - 1, torch.full_like(ids, arch.CLAP_TEXT["eos_id"]), ids)
+    ids = torch.where(pos < n, ids, torch.full_like(ids, arch.CLAP_TEXT["pad_id"]))
+    return ids.to(device), (pos < n).float().to(device)
+
+
 def encoder_outputs(batch: int, t5_lens, seed: int = 78, device="cpu"):
     """Synthetic encoder outputs for the sequence-generation models (SURVEY.md 8d): CLAP [B, 1, 512] L2-normalised (as
     the CLAP embedding is), Flan-T5 hidden states [B, L, 1024] N(0, 1) with L = max(t5_lens) and the padding mask of

@@ -30,6 +30,9 @@
  *       encoders/modules.py:271-300                                ALDM_OP_KV_ATTN, ALDM_OP_SEQ_FEEDBACK)
  *   FlanT5HiddenState.encode_text -> T5EncoderModel (from the      aldm_program_run(t5 program: embedding + 24
  *       token ids)  encoders/modules.py:113-198                    blocks; ALDM_OP_T5_EMBED .. ALDM_OP_T5_GATE)
+ *   CLAP.get_text_embedding (RoBERTa text branch, pooler,         aldm_program_run(clap program: embedding + LN +
+ *       text_projection, F.normalize) clap/open_clip/model.py:     12 blocks + head; ALDM_OP_CLAP_EMBED ..
+ *       656-663,730-750; encoders/modules.py:660-735               ALDM_OP_CLAP_HEAD)
  *
  * Conventions
  *   - all pointers are DEVICE pointers unless named host_*; buffers are caller-owned (torch
@@ -53,7 +56,7 @@
 extern "C" {
 #endif
 
-#define ALDM_ABI_VERSION 10
+#define ALDM_ABI_VERSION 11
 #define ALDM_MAX_TAPS 16
 
 enum {
@@ -330,12 +333,77 @@ typedef struct aldm_t5_gate_desc {
 } aldm_t5_gate_desc;
 int aldm_t5_gate(const aldm_t5_gate_desc* d, void* stream);
 
+/* ---- CLAP text branch from token ids (csrc/clap/clap_text.cu) --------------------------------
+ * RoBERTa-base, post-LN: the residual stream is the fp32 output of each LayerNorm, [B * L, C]; every projection is a
+ * two-plane GEMM.  Sequences hold at most 512 tokens (the tokenizer's max_length), heads of 64. */
+
+/* out[b * L + t, :] = (word[id] + type[0]) + pos[pid] with HF's position ids, computed from the ids:
+ * pid = (number of ids != pad among ids[b, 0..t]) * (id != pad) + pad.  The host checks 0 <= id < vocab; an id outside
+ * that range (or a pid >= n_pos) writes a NaN row.  L > 512 is ALDM_E_SHAPE. */
+typedef struct aldm_clap_embed_desc {
+  const int64_t* ids;        /* [B, L] */
+  const float* word;         /* [vocab, C] */
+  const float* pos;          /* [n_pos, C] */
+  const float* type;         /* [C]: token_type_embeddings row 0 */
+  float* out;                /* [B * L, C] */
+  int32_t B, L, vocab, n_pos, C, pad;
+} aldm_clap_embed_desc;
+int aldm_clap_embed(const aldm_clap_embed_desc* d, void* stream);
+
+/* LayerNorm per row of C (C % 128 == 0, <= 1024): two-pass fp32 statistics in a fixed order, y = (x - mean) * rstd *
+ * gamma + beta.  Writes BOTH fp32 out_f32 [rows, C] (the post-LN residual stream) and operand planes out_hi / out_lo
+ * [rows, ldo] for the next GEMM. */
+typedef struct aldm_clap_ln_desc {
+  const float* x;            /* [rows, C] */
+  const float* gamma;        /* [C] */
+  const float* beta;         /* [C] */
+  float* out_f32;
+  void* out_hi; void* out_lo;
+  int32_t rows, C, ldo;
+  float eps;
+} aldm_clap_ln_desc;
+int aldm_clap_layernorm(const aldm_clap_ln_desc* d, void* stream);
+
+/* Bidirectional self-attention of B sequences of L <= 512 tokens: s[i, j] = (q_i . k_j) / 8; keys with mask[b, j] != 1
+ * get probability exactly 0 (at least one key per row must be valid); fp32 softmax and P V.  qkv [B * L, ld_qkv] holds
+ * q | k | v at columns [0, C), [C, 2C), [2C, 3C), head h at [h*64, +64).  Output: planes [B * L, ldo].  L > 512 or
+ * heads * 64 != C is ALDM_E_SHAPE. */
+typedef struct aldm_clap_attn_desc {
+  const float* qkv;
+  const float* mask;         /* [B, L] */
+  void* out_hi; void* out_lo;
+  int32_t B, L, heads, C, ld_qkv, ldo;
+} aldm_clap_attn_desc;
+int aldm_clap_attention(const aldm_clap_attn_desc* d, void* stream);
+
+/* erf-GELU: y[r, c] = 0.5 x (1 + erf(x / sqrt(2))) of x = the fp32 output of the intermediate GEMM (bias added), c < F,
+ * written as operand planes [rows, ldo]. */
+typedef struct aldm_clap_gelu_desc {
+  const float* x;            /* [rows, ld_x] */
+  void* out_hi; void* out_lo;
+  int32_t rows, F, ld_x, ldo;
+} aldm_clap_gelu_desc;
+int aldm_clap_gelu(const aldm_clap_gelu_desc* d, void* stream);
+
+/* Per batch row b, fp32: p = tanh(Wp x[b * L] + bp) (the pooler, token 0), t = relu(W1 p + b1), y = W2 t + b2,
+ * out[b] = y / max(||y||_2, 1e-12).  Weights are stored transposed ([in, out], row-major).  C, P <= 1024. */
+typedef struct aldm_clap_head_desc {
+  const float* x;            /* [B * L, C]: the last LayerNorm's fp32 output */
+  const float* wp_t; const float* bp;     /* [C, C], [C] */
+  const float* w1_t; const float* b1;     /* [C, P], [P] */
+  const float* w2_t; const float* b2;     /* [P, P], [P] */
+  float* out;                /* [B, P] */
+  int32_t B, L, C, P;
+} aldm_clap_head_desc;
+int aldm_clap_head(const aldm_clap_head_desc* d, void* stream);
+
 /* ---- programs: flat op tables replayed on a stream / as a CUDA graph ---------------------- */
 
 enum { ALDM_OP_GEMM = 1, ALDM_OP_PREP = 2, ALDM_OP_ATTN = 3, ALDM_OP_SOFTMAX = 4, ALDM_OP_TEMB = 5,
        ALDM_OP_TRANSPOSE = 6, ALDM_OP_PACKB = 7, ALDM_OP_COPY = 8, ALDM_OP_SEQ_ASSEMBLE = 9, ALDM_OP_KV_ATTN = 10,
        ALDM_OP_SEQ_FEEDBACK = 11, ALDM_OP_T5_EMBED = 12, ALDM_OP_T5_RMSNORM = 13, ALDM_OP_T5_ATTN = 14,
-       ALDM_OP_T5_GATE = 15 };
+       ALDM_OP_T5_GATE = 15, ALDM_OP_CLAP_EMBED = 16, ALDM_OP_CLAP_LN = 17, ALDM_OP_CLAP_ATTN = 18,
+       ALDM_OP_CLAP_GELU = 19, ALDM_OP_CLAP_HEAD = 20 };
 
 typedef struct aldm_op {
   int32_t kind;
@@ -356,6 +424,11 @@ typedef struct aldm_op {
     aldm_t5_rmsnorm_desc t5_rmsnorm;
     aldm_t5_attn_desc t5_attn;
     aldm_t5_gate_desc t5_gate;
+    aldm_clap_embed_desc clap_embed;
+    aldm_clap_ln_desc clap_ln;
+    aldm_clap_attn_desc clap_attn;
+    aldm_clap_gelu_desc clap_gelu;
+    aldm_clap_head_desc clap_head;
   } u;
 } aldm_op;
 
