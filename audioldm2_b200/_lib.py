@@ -17,7 +17,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libaldm_b200.so")
 SOURCES = ["gemm.cu", "prep.cu", "attention.cu", "elementwise.cu", "stft.cu", "program.cu", "engine_abi.cu", "microbench.cu",
-           "cond/seqgen.cu", "text/t5.cu", "clap/clap_text.cu"]
+           "cond/seqgen.cu", "text/t5.cu", "clap/clap_text.cu", "audio/htsat.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
@@ -25,7 +25,7 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-
 NVCC = shutil.which("nvcc") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
 
 MAX_TAPS = 16
-ABI_VERSION = 11
+ABI_VERSION = 12
 
 # enums (keep in sync with the header; checked by tests/test_abi.py against the header text)
 GEMM_TC, GEMM_SIMT, GEMM_TC_V1 = 0, 1, 2
@@ -41,6 +41,7 @@ OP_GEMM, OP_PREP, OP_ATTN, OP_SOFTMAX, OP_TEMB, OP_TRANSPOSE, OP_PACKB, OP_COPY 
 OP_SEQ_ASSEMBLE, OP_KV_ATTN, OP_SEQ_FEEDBACK = 9, 10, 11
 OP_T5_EMBED, OP_T5_RMSNORM, OP_T5_ATTN, OP_T5_GATE = 12, 13, 14, 15
 OP_CLAP_EMBED, OP_CLAP_LN, OP_CLAP_ATTN, OP_CLAP_GELU, OP_CLAP_HEAD = 16, 17, 18, 19, 20
+OP_HTSAT_LOGMEL, OP_HTSAT_PATCH, OP_HTSAT_ATTN, OP_HTSAT_MERGE, OP_HTSAT_HEAD = 21, 22, 23, 24, 25
 
 
 class GemmDesc(C.Structure):
@@ -176,13 +177,43 @@ class ClapHeadDesc(C.Structure):
                 ("B", C.c_int32), ("L", C.c_int32), ("C", C.c_int32), ("P", C.c_int32)]
 
 
+class HtsatLogmelDesc(C.Structure):
+    _fields_ = [("wav", C.c_void_p), ("taps", C.c_void_p), ("melW", C.c_void_p), ("bn_mean", C.c_void_p),
+                ("bn_var", C.c_void_p), ("bn_w", C.c_void_p), ("bn_b", C.c_void_p), ("out", C.c_void_p),
+                ("n", C.c_int32), ("L", C.c_int32), ("up", C.c_int32), ("L48", C.c_int32), ("T", C.c_int32),
+                ("eps", C.c_float)]
+
+
+class HtsatPatchDesc(C.Structure):
+    _fields_ = [("mel", C.c_void_p), ("w", C.c_void_p), ("bias", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p),
+                ("out", C.c_void_p), ("n", C.c_int32), ("T", C.c_int32), ("eps", C.c_float)]
+
+
+class HtsatAttnDesc(C.Structure):
+    _fields_ = [("qkv", C.c_void_p), ("bias", C.c_void_p), ("mask", C.c_void_p), ("out_hi", C.c_void_p),
+                ("out_lo", C.c_void_p), ("n", C.c_int32), ("R", C.c_int32), ("shift", C.c_int32), ("heads", C.c_int32),
+                ("head_dim", C.c_int32), ("C", C.c_int32), ("ld_qkv", C.c_int32), ("ldo", C.c_int32), ("scale", C.c_float)]
+
+
+class HtsatMergeDesc(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p), ("out_hi", C.c_void_p), ("out_lo", C.c_void_p),
+                ("n", C.c_int32), ("R", C.c_int32), ("C", C.c_int32), ("ldo", C.c_int32), ("eps", C.c_float)]
+
+
+class HtsatHeadDesc(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p), ("w1_t", C.c_void_p), ("b1", C.c_void_p),
+                ("w2_t", C.c_void_p), ("b2", C.c_void_p), ("out", C.c_void_p),
+                ("n", C.c_int32), ("ntok", C.c_int32), ("C", C.c_int32), ("P", C.c_int32), ("eps", C.c_float)]
+
+
 class _OpU(C.Union):
     _fields_ = [("gemm", GemmDesc), ("prep", PrepDesc), ("attn", AttnDesc), ("softmax", _Softmax),
                 ("temb", _Temb), ("transpose", _Transpose), ("packb", _PackB), ("copy", _Copy),
                 ("seq_assemble", SeqAssembleDesc), ("kv_attn", KvAttnDesc), ("seq_feedback", SeqFeedbackDesc),
                 ("t5_embed", T5EmbedDesc), ("t5_rmsnorm", T5RmsnormDesc), ("t5_attn", T5AttnDesc), ("t5_gate", T5GateDesc),
                 ("clap_embed", ClapEmbedDesc), ("clap_ln", ClapLnDesc), ("clap_attn", ClapAttnDesc), ("clap_gelu", ClapGeluDesc),
-                ("clap_head", ClapHeadDesc)]
+                ("clap_head", ClapHeadDesc), ("htsat_logmel", HtsatLogmelDesc), ("htsat_patch", HtsatPatchDesc),
+                ("htsat_attn", HtsatAttnDesc), ("htsat_merge", HtsatMergeDesc), ("htsat_head", HtsatHeadDesc)]
 
 
 class Op(C.Structure):
@@ -271,6 +302,11 @@ def lib() -> C.CDLL:
         "aldm_clap_attention": (i32, [C.POINTER(ClapAttnDesc), vp]),
         "aldm_clap_gelu": (i32, [C.POINTER(ClapGeluDesc), vp]),
         "aldm_clap_head": (i32, [C.POINTER(ClapHeadDesc), vp]),
+        "aldm_htsat_logmel": (i32, [C.POINTER(HtsatLogmelDesc), vp]),
+        "aldm_htsat_patch": (i32, [C.POINTER(HtsatPatchDesc), vp]),
+        "aldm_htsat_window_attention": (i32, [C.POINTER(HtsatAttnDesc), vp]),
+        "aldm_htsat_merge": (i32, [C.POINTER(HtsatMergeDesc), vp]),
+        "aldm_htsat_head": (i32, [C.POINTER(HtsatHeadDesc), vp]),
         "aldm_softmax_rows": (i32, [vp, i32, i32, f32, vp, vp, vp]),
         "aldm_timestep_embedding": (i32, [vp, i32, i32, vp, vp, vp, vp]),
         "aldm_ddim_step": (i32, [vp, vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, vp]),
@@ -323,6 +359,7 @@ EXPORTED = ["aldm_gemm", "aldm_gemm_variant", "aldm_gemm_a_mode", "aldm_prep", "
             "aldm_kv_attention", "aldm_seq_assemble", "aldm_seq_feedback",
             "aldm_t5_embed", "aldm_t5_rmsnorm", "aldm_t5_attention", "aldm_t5_gate",
             "aldm_clap_embed", "aldm_clap_layernorm", "aldm_clap_attention", "aldm_clap_gelu", "aldm_clap_head",
+            "aldm_htsat_logmel", "aldm_htsat_patch", "aldm_htsat_window_attention", "aldm_htsat_merge", "aldm_htsat_head",
             "aldm_timestep_embedding", "aldm_ddim_step", "aldm_masked_blend", "aldm_transpose_chw",
             "aldm_posterior_sample", "aldm_stft_mel", "aldm_program_create", "aldm_program_run",
             "aldm_program_run_range", "aldm_program_capture", "aldm_program_replay",

@@ -480,3 +480,66 @@ def has_clap(cfg: dict) -> bool:
     """Configs conditioned on the CLAP text embedding: audioldm2-full / -large (GPT-2's first input) and audioldm_48k (the
     FiLM vector, 512 wide).  The tiny FiLM test configs (dim 24) are not."""
     return has_seqgen(cfg) or cfg["unet"].get("extra_film_condition_dim") == CLAP_TEXT["joint_dim"]
+
+
+# --------------------------------------------------------------------------------------
+# CLAP audio branch (CLAPAudioEmbeddingClassifierFreev2 with embed_mode "audio", encoders/modules.py:689-716, and
+# CLAP.get_audio_embedding, clap/open_clip/model.py:752-777): HTSAT-base (HTSAT_Swin_Transformer, clap/open_clip/htsat.py,
+# config :1271-1284 and model_configs/HTSAT-base.json) without fusion -- torchlibrosa's Spectrogram (n_fft 1024, hop 480,
+# periodic Hann, reflect-centred) and LogmelFilterBank (64 mel bins, 50 Hz - 14 kHz, 10 log10, ref 1, no top_db), bn0,
+# reshape_wav2img to a 256 x 256 image, a 4 x 4 patch embedding to a 64 x 64 grid of 128 channels, four pre-LN Swin stages
+# (depths 2, 2, 12, 2; heads 4, 8, 16, 32 of 32 dims; 8 x 8 windows, odd blocks shifted by 4 where the grid is larger than
+# a window) joined by PatchMerging, the final LayerNorm(1024) and the mean over tokens -- then audio_projection (Linear
+# 1024 -> 512, ReLU, Linear 512 -> 512) and F.normalize.  Input: 48 kHz audio, resampled from 16 kHz by torchaudio first,
+# truncated to 480 000 samples.
+# --------------------------------------------------------------------------------------
+
+CLAP_AUDIO = dict(sample_rate=48000, n_fft=1024, hop=480, n_mels=64, fmin=50.0, fmax=14000.0, max_samples=480000,
+                  spec_size=256, freq_ratio=4, frames=1024, patch=4, embed_dim=128, depths=(2, 2, 12, 2),
+                  heads=(4, 8, 16, 32), head_dim=32, window=8, mlp_ratio=4, eps=1e-5, joint_dim=512, bn_eps=1e-5)
+
+
+def clap_audio_param_shapes(depths=CLAP_AUDIO["depths"]) -> Dict[str, Tuple[int, ...]]:
+    """name -> shape of the CLAP audio branch's parameters and the running statistics of bn0 (relative to the CLAP model,
+    e.g. ``clap.model.``): ``audio_branch.`` (HTSAT_Swin_Transformer, torchlibrosa's extractors included) and
+    ``audio_projection.{0,2}``.  The relative_position_index / attn_mask buffers, tscam_conv and head are not read."""
+    A = CLAP_AUDIO
+    nb, E, M = A["n_fft"] // 2 + 1, A["embed_dim"], A["n_mels"]
+    a = "audio_branch"
+    S: Dict[str, Tuple[int, ...]] = {
+        f"{a}.spectrogram_extractor.stft.conv_real.weight": (nb, 1, A["n_fft"]),
+        f"{a}.spectrogram_extractor.stft.conv_imag.weight": (nb, 1, A["n_fft"]),
+        f"{a}.logmel_extractor.melW": (nb, M),
+        f"{a}.bn0.weight": (M,), f"{a}.bn0.bias": (M,), f"{a}.bn0.running_mean": (M,), f"{a}.bn0.running_var": (M,),
+        f"{a}.patch_embed.proj.weight": (E, 1, A["patch"], A["patch"]), f"{a}.patch_embed.proj.bias": (E,),
+        f"{a}.patch_embed.norm.weight": (E,), f"{a}.patch_embed.norm.bias": (E,),
+    }
+    nrel = (2 * A["window"] - 1) ** 2
+    for i, depth in enumerate(depths):
+        C, H = E * 2 ** i, A["heads"][i]
+        for j in range(depth):
+            b = f"{a}.layers.{i}.blocks.{j}"
+            S[f"{b}.norm1.weight"] = (C,); S[f"{b}.norm1.bias"] = (C,)
+            S[f"{b}.attn.relative_position_bias_table"] = (nrel, H)
+            S[f"{b}.attn.qkv.weight"] = (3 * C, C); S[f"{b}.attn.qkv.bias"] = (3 * C,)
+            S[f"{b}.attn.proj.weight"] = (C, C); S[f"{b}.attn.proj.bias"] = (C,)
+            S[f"{b}.norm2.weight"] = (C,); S[f"{b}.norm2.bias"] = (C,)
+            S[f"{b}.mlp.fc1.weight"] = (A["mlp_ratio"] * C, C); S[f"{b}.mlp.fc1.bias"] = (A["mlp_ratio"] * C,)
+            S[f"{b}.mlp.fc2.weight"] = (C, A["mlp_ratio"] * C); S[f"{b}.mlp.fc2.bias"] = (C,)
+        if i < len(depths) - 1:
+            d = f"{a}.layers.{i}.downsample"
+            S[f"{d}.norm.weight"] = (4 * C,); S[f"{d}.norm.bias"] = (4 * C,)
+            S[f"{d}.reduction.weight"] = (2 * C, 4 * C)
+    F = E * 2 ** (len(depths) - 1)
+    S[f"{a}.norm.weight"] = (F,); S[f"{a}.norm.bias"] = (F,)
+    P = A["joint_dim"]
+    S["audio_projection.0.weight"] = (P, F); S["audio_projection.0.bias"] = (P,)
+    S["audio_projection.2.weight"] = (P, P); S["audio_projection.2.bias"] = (P,)
+    return S
+
+
+def clap_audio_frames(n_samples: int, sampling_rate: int) -> int:
+    """Frames T of the spectrogram of an n-sample clip at ``sampling_rate`` (16 000 or 48 000): the 48 kHz length
+    (3 n at 16 kHz, torchaudio's ceil(3 n / 1)) truncated to 480 000 samples, // 480 + 1."""
+    L48 = min(n_samples * (48000 // sampling_rate), CLAP_AUDIO["max_samples"])
+    return L48 // CLAP_AUDIO["hop"] + 1

@@ -120,3 +120,104 @@ class NativeCLAPTextEncoder:
         if self._uncond is None:
             self._uncond = self.embed(*empty_prompt(1, 2, self.device))
         return self._uncond
+
+
+class NativeCLAPAudioEncoder:
+    """The CLAP audio embedding, run natively from the waveform: ``embed(waveform [n, L])`` returns what the reference's
+    CLAPAudioEmbeddingClassifierFreev2 computes in audio mode before its random replacement (encoders/modules.py:689-716):
+    torchaudio's resample to 48 kHz unless ``sampling_rate`` is 48 000, the truncation to 480 000 samples, then
+    CLAP.get_audio_embedding with the HTSAT-base branch -- [n, 512] float32 on the device, L2-normalised.
+
+    Every kernel is sm_90a code of this package (plan.build_clap_audio: the log-mel front end, the patch embedding, 18 Swin
+    blocks, 3 PatchMergings and the head), one op table per (n, L, sampling rate) replayed as a CUDA graph; plans are built
+    lazily and the two most recent are kept, sharing one uploaded weight arena.  Nothing is read back after a run:
+    pack_clap_audio_weights has already ruled out values beyond the fp16 range of the operand planes from the weights."""
+
+    def __init__(self, state_dict: Optional[Dict[str, torch.Tensor]] = None, device="cuda:0", sampling_rate: int = 16000,
+                 use_graph: bool = True, max_plans: int = 2, weights: Optional[plan.ClapAudioWeights] = None):
+        if not torch.cuda.is_available():
+            raise RuntimeError("the native CLAP audio encoder needs a CUDA device (sm_90a); there is no CPU fallback")
+        if int(sampling_rate) not in (16000, 48000):
+            raise ValueError(f"CLAP audio encoder: sampling rate {sampling_rate} (16000 or 48000)")
+        self.device = torch.device(device)
+        self.sampling_rate = int(sampling_rate)
+        self.use_graph = use_graph
+        self.max_plans = max_plans
+        self.weights = weights if weights is not None else plan.pack_clap_audio_weights(state_dict)
+        self.arena = self.weights.arena.to(self.device)
+        self._progs: "OrderedDict[tuple, engine.DeviceProgram]" = OrderedDict()
+
+    def check(self, waveform: torch.Tensor):
+        """Raise ValueError unless waveform is a float32 [n, L] tensor whose 48 kHz signal is longer than 512 samples
+        (reflect padding of the first frame)."""
+        if waveform.dim() != 2 or waveform.dtype != torch.float32:
+            raise ValueError(f"waveform must be a float32 tensor [n, L], got {waveform.dtype} {tuple(waveform.shape)}")
+        n, L = waveform.shape
+        L48 = min(L * (48000 // self.sampling_rate), arch.CLAP_AUDIO["max_samples"])
+        if n < 1 or L48 <= arch.CLAP_AUDIO["n_fft"] // 2:
+            raise ValueError(f"waveform [n={n}, L={L}] at {self.sampling_rate} Hz: need n >= 1 and more than "
+                             f"{arch.CLAP_AUDIO['n_fft'] // 2} samples at 48 kHz")
+
+    def program(self, n: int, L: int) -> engine.DeviceProgram:
+        key = (int(n), int(L), self.sampling_rate)
+        prog = self._progs.get(key)
+        if prog is not None:
+            self._progs.move_to_end(key)
+            return prog
+        while len(self._progs) >= self.max_plans:
+            self._progs.popitem(last=False)[1].close()
+        pl = plan.build_clap_audio(None, n, L, self.sampling_rate, weights=self.weights)
+        prog = engine.DeviceProgram(pl, self.device, dict(all=(pl.marks["begin"], pl.marks["end"])), arena_dev=self.arena)
+        self._progs[key] = prog
+        return prog
+
+    @torch.no_grad()
+    def embed(self, waveform: torch.Tensor) -> torch.Tensor:
+        """waveform [n, L] float32 (host or device) -> the audio embedding [n, 512] float32 on the device."""
+        self.check(waveform)
+        prog = self.program(*waveform.shape)
+        prog.view("wav").copy_(waveform)
+        if self.use_graph:
+            prog.replay("all")
+        else:
+            prog.run("all")
+        return prog.view("embed").clone()
+
+
+def replacement_draws(n: int) -> list:
+    """The draws of CLAPAudioEmbeddingClassifierFreev2.forward after an embedding of n rows (encoders/modules.py:730-733):
+    one torch.rand(1) per row in row order; a row is replaced by CLAP("") below unconditional_prob = 0.1.  Used for the
+    conditioning rows (pipeline.clap_replacement_draws) and for both halves of the ranker's cos_similarity."""
+    return [float(torch.rand(1)) < 0.1 for _ in range(n)]
+
+
+class NativeCLAPRanker:
+    """The reference's re-ranker ``clap.cos_similarity(waveform, text)`` (encoders/modules.py:639-653, ddpm.py:1554-1568),
+    natively: ``__call__(waveform [n, L], texts) -> similarity [n]`` on the device, the contract of the pipeline's ``ranker``
+    hook.  The audio rows are embedded, then forward's n draws replace rows by CLAP(""); the texts are tokenized by
+    ``tokenize(texts) -> (ids, mask)`` (the RoBERTa tokenizer stays with the caller) and embedded, then n more draws; then
+    the cosine similarity.  ``rows`` / ``n_total`` rank a subset of a larger call (one rank of a sharded call): all
+    2 n_total draws are made, in global row order, and row k of ``waveform`` takes the decisions of global row rows[k]."""
+
+    def __init__(self, audio_encoder: NativeCLAPAudioEncoder, text_encoder: NativeCLAPTextEncoder, tokenize):
+        self.audio, self.text, self.tokenize = audio_encoder, text_encoder, tokenize
+
+    @torch.no_grad()
+    def __call__(self, waveform: torch.Tensor, texts, rows=None, n_total: Optional[int] = None) -> torch.Tensor:
+        n = waveform.shape[0]
+        if len(texts) != n:
+            raise ValueError(f"{len(texts)} texts for {n} waveforms")
+        rows = list(range(n)) if rows is None else [int(r) for r in rows]
+        n_total = n if n_total is None else int(n_total)
+        u = self.text.unconditional()
+        a = self.audio.embed(waveform)
+        da = replacement_draws(n_total)
+        ra = [k for k, g in enumerate(rows) if da[g]]
+        if ra:
+            a[ra] = u
+        t = self.text.embed(*self.tokenize(list(texts)))
+        dt = replacement_draws(n_total)
+        rt = [k for k, g in enumerate(rows) if dt[g]]
+        if rt:
+            t[rt] = u.to(t.device)
+        return torch.nn.functional.cosine_similarity(a[:, None], t[:, None], dim=2).reshape(-1)

@@ -56,6 +56,11 @@ int clap_layernorm_launch(const aldm_clap_ln_desc& d, cudaStream_t st);
 int clap_attention_launch(const aldm_clap_attn_desc& d, cudaStream_t st);
 int clap_gelu_launch(const aldm_clap_gelu_desc& d, cudaStream_t st);
 int clap_head_launch(const aldm_clap_head_desc& d, cudaStream_t st);
+int htsat_logmel_launch(const aldm_htsat_logmel_desc& d, cudaStream_t st);
+int htsat_patch_launch(const aldm_htsat_patch_desc& d, cudaStream_t st);
+int htsat_window_attention_launch(const aldm_htsat_attn_desc& d, cudaStream_t st);
+int htsat_merge_launch(const aldm_htsat_merge_desc& d, cudaStream_t st);
+int htsat_head_launch(const aldm_htsat_head_desc& d, cudaStream_t st);
 
 }  // namespace aldm
 
@@ -96,6 +101,11 @@ static int run_op(const aldm_op& op, cudaStream_t st) {
     case ALDM_OP_CLAP_ATTN: return clap_attention_launch(op.u.clap_attn, st);
     case ALDM_OP_CLAP_GELU: return clap_gelu_launch(op.u.clap_gelu, st);
     case ALDM_OP_CLAP_HEAD: return clap_head_launch(op.u.clap_head, st);
+    case ALDM_OP_HTSAT_LOGMEL: return htsat_logmel_launch(op.u.htsat_logmel, st);
+    case ALDM_OP_HTSAT_PATCH: return htsat_patch_launch(op.u.htsat_patch, st);
+    case ALDM_OP_HTSAT_ATTN: return htsat_window_attention_launch(op.u.htsat_attn, st);
+    case ALDM_OP_HTSAT_MERGE: return htsat_merge_launch(op.u.htsat_merge, st);
+    case ALDM_OP_HTSAT_HEAD: return htsat_head_launch(op.u.htsat_head, st);
     case ALDM_OP_COPY:
       ALDM_CHECK_CUDA(cudaMemcpyAsync(op.u.copy.dst, op.u.copy.src, (size_t)op.u.copy.bytes, cudaMemcpyDeviceToDevice, st));
       return ALDM_OK;

@@ -21,8 +21,9 @@ CUDA graph (csrc/engine_abi.cu).
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
-from typing import Dict, List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -99,6 +100,42 @@ def split_clap_text_state_dict(state_dict: Dict[str, torch.Tensor], prefix: str)
         if tuple(v.shape) != tuple(shp):
             raise ValueError(f"{prefix + k}: shape {tuple(v.shape)}, expected {shp}")
         out[k] = v
+    return out
+
+
+def htsat_dft_basis(n_fft: int = 1024) -> Tuple[torch.Tensor, torch.Tensor]:
+    """torchlibrosa's STFT conv weights (DFTBase.dft_matrix times the periodic Hann window): real[k, 0, n] =
+    cos(2 pi k n / N) w[n], imag[k, 0, n] = -sin(2 pi k n / N) w[n], k = 0 .. N / 2, in float64."""
+    nn_ = torch.arange(n_fft, dtype=torch.float64)
+    k = torch.arange(n_fft // 2 + 1, dtype=torch.float64)
+    win = 0.5 - 0.5 * torch.cos(2 * math.pi * nn_ / n_fft)
+    ph = 2 * math.pi * ((k[:, None] * nn_[None, :]) % n_fft) / n_fft
+    return (torch.cos(ph) * win)[:, None, :], (-torch.sin(ph) * win)[:, None, :]
+
+
+def split_clap_audio_state_dict(state_dict: Dict[str, torch.Tensor], prefix: str) -> Dict[str, torch.Tensor]:
+    """The CLAP audio branch's weights from a reference checkpoint: the keys under ``prefix`` (the CLAP model, e.g.
+    ``clap.model.``), named and shaped as arch.clap_audio_param_shapes, with as many Swin blocks per stage as the
+    checkpoint holds.  tscam_conv, head, the relative_position_index / attn_mask buffers, bn0.num_batches_tracked and the
+    text branch are ignored.  The log-mel filterbank is the checkpoint's melW; the STFT weights must be torchlibrosa's
+    periodic-Hann DFT basis (the native front end computes an FFT instead of reading them).  Raises KeyError for a missing
+    key, ValueError for a wrong shape or a different STFT basis."""
+    depths = plan.htsat_depths(state_dict, prefix)
+    out = {}
+    for k, shp in arch.clap_audio_param_shapes(tuple(depths)).items():
+        v = state_dict.get(prefix + k)
+        if v is None:
+            raise KeyError(f"checkpoint has no {prefix + k} (needed by the CLAP audio encoder)")
+        if tuple(v.shape) != tuple(shp):
+            raise ValueError(f"{prefix + k}: shape {tuple(v.shape)}, expected {shp}")
+        out[k] = v
+    real, imag = htsat_dft_basis(arch.CLAP_AUDIO["n_fft"])
+    for name, ref in (("conv_real", real), ("conv_imag", imag)):
+        k = f"audio_branch.spectrogram_extractor.stft.{name}.weight"
+        err = float((out[k].double() - ref).abs().max())
+        if not err <= 1e-6:
+            raise ValueError(f"{prefix + k} differs from the periodic-Hann DFT basis by {err:.3g}: the native front end "
+                             "computes that transform as an FFT and cannot use other STFT weights")
     return out
 
 

@@ -19,9 +19,12 @@ network.  What differs, by design of this tier:
   tokenizer's output under the reference's key, ``film_clap_cond1`` = [input_ids (integer) [B, L], attention_mask [B, L]]:
   the embedding is then computed natively (clap.NativeCLAPTextEncoder) before everything else, with the reference's random
   replacement of prompt rows by CLAP("") (clap_replacement_draws);
-* candidate re-ranking (ddpm.py:1554-1568) uses ``latent_diffusion.ranker(waveform [n,1,L], texts) -> similarity [n]``
-  (the reference's ``clap.cos_similarity``); without one the first candidate of each prompt is returned and a
-  warning says so;
+* candidate re-ranking (ddpm.py:1554-1568) is the reference's ``clap.cos_similarity``, run natively
+  (clap.NativeCLAPRanker: the HTSAT audio branch and the RoBERTa text branch of ``clap.model.*``, with forward's random
+  replacement by CLAP("")) when the model is built with ``clap_tokenize=`` (the caller's RoBERTa tokenizer); it ranks the
+  waveforms on the device and only the selected ones are copied to the host.  Otherwise a Python
+  ``latent_diffusion.ranker(waveform [n,1,L], texts) -> similarity [n]`` may be attached; without either the first
+  candidate of each prompt is returned and a warning says so;
 * the engine is planned per (latent batch, latent length); ``NativeAudioLDM2.engine`` re-plans on demand and caches.
 """
 from __future__ import annotations
@@ -150,9 +153,10 @@ def clap_replacement_draws(n: int, extra: bool) -> list:
     model after its first: conditional_dry_run_finished) LatentDiffusion.make_decision(0.0) draws one torch.rand(1)
     (ddpm.py:852-854); then CLAPAudioEmbeddingClassifierFreev2.forward draws one per prompt row, in row order, and replaces
     the row by CLAP("") below unconditional_prob = 0.1 (encoders/modules.py:731-733).  -> the n decisions."""
+    from .clap import replacement_draws
     if extra:
         torch.rand(1)                               # make_decision(0.0): drawn, never true
-    return [float(torch.rand(1)) < 0.1 for _ in range(n)]
+    return replacement_draws(n)
 
 
 def encode_clap_tokens(cfg: dict, cond: dict, encoder: Callable[[], object], unconditional: bool = False,
@@ -257,10 +261,17 @@ class NativeAudioLDM2:
 
     def __init__(self, cfg: dict, unet_sd, vae_sd, vocoder_sd, device, scale_factor: float = 1.0, ctx_max_len=None,
                  cond_provider=None, ranker: Optional[Callable] = None, seqgen_sd=None, t5_sd=None, t5_uncond_sd=None,
-                 clap_sd=None, **engine_kw):
+                 clap_sd=None, clap_rank_sd=None, clap_tokenize=None, **engine_kw):
         """``t5_sd`` / ``t5_uncond_sd``: the Flan-T5 weights of the conditional and of the unconditional branch (or callables
         that return them, for weights made on first use); ``t5_uncond_sd`` None means the same weights.  ``clap_sd``: the
-        CLAP text branch's weights (or a callable)."""
+        CLAP text branch's weights (or a callable).  ``clap_tokenize``: the RoBERTa tokenizer, ``texts -> (ids, mask)``; with
+        it candidates are ranked natively by the weights of ``clap_rank_sd``, (audio branch, text branch) of the reference's
+        ``clap.model``, each a state dict or a callable that returns one."""
+        if ranker is not None and clap_tokenize is not None:
+            raise ValueError("pass either a ranker or clap_tokenize (the native CLAP ranker), not both")
+        if clap_tokenize is not None and cfg.get("sampling_rate") not in (16000, 48000):
+            raise ValueError(f"{cfg.get('name')}: the native CLAP ranker takes 16 or 48 kHz audio, "
+                             f"not {cfg.get('sampling_rate')} Hz")
         self.cfg, self.device = cfg, torch.device(device)
         self._sd = (unet_sd, vae_sd, vocoder_sd)
         self.scale_factor = scale_factor
@@ -277,6 +288,8 @@ class NativeAudioLDM2:
         self._t5 = None
         self._clap_sd = clap_sd
         self._clap = None
+        self._clap_rank_sd, self.clap_tokenize = clap_rank_sd, clap_tokenize
+        self._native_ranker = None
         self.conditional_dry_run_finished = False           # LatentDiffusion's flag (ddpm.py:852-854, 916-917)
 
     # ---- AudioMAE token generator (built on first use: UNet-boundary providers never pay for it) ----------------------
@@ -317,6 +330,29 @@ class NativeAudioLDM2:
             from .clap import NativeCLAPTextEncoder
             self._clap = NativeCLAPTextEncoder(self._clap_sd() if callable(self._clap_sd) else self._clap_sd, self.device)
         return self._clap
+
+    # ---- native CLAP re-ranker (built on the first call with n_gen > 1) ------------------------------------------
+    def native_ranker(self):
+        """clap.NativeCLAPRanker over the reference's ``clap.model``.  Its text branch shares the conditioning CLAP text
+        encoder (arena and cached CLAP("")) when the two weight sets are equal."""
+        if self._native_ranker is None:
+            from .clap import NativeCLAPAudioEncoder, NativeCLAPRanker, NativeCLAPTextEncoder
+            get = lambda w: w() if callable(w) else w
+            src_a, src_t = self._clap_rank_sd
+            text = None
+            if self._clap_sd is not None:
+                if src_t is self._clap_sd:                  # the same weights, or the same generator of synthetic ones
+                    text = self.clap_encoder()
+                elif not callable(src_t) and not callable(self._clap_sd):
+                    sd_c = self._clap_sd
+                    if set(sd_c) == set(src_t) and all(torch.equal(sd_c[k], src_t[k]) for k in src_t):
+                        text = self.clap_encoder()
+            if text is None:
+                text = NativeCLAPTextEncoder(get(src_t), self.device)
+            sd_a = get(src_a)
+            audio = NativeCLAPAudioEncoder(sd_a, self.device, sampling_rate=self.cfg["sampling_rate"])
+            self._native_ranker = NativeCLAPRanker(audio, text, self.clap_tokenize)
+        return self._native_ranker
 
     def conditioning(self, batch) -> dict:
         """The provider's conditioning of the call's B prompts, as the reference's get_input makes it (after the posterior
@@ -442,6 +478,13 @@ class NativeAudioLDM2:
         texts = list(batch["text"]) * n_gen
         wave = eng.generate_waveform(cond, uncond, ddim_steps=ddim_steps, guidance=guidance, eta=ddim_eta, mask=mask, x0=x0,
                                      x_T=x_T, noise_fn=noise_fn)
+        if n_gen > 1 and self.clap_tokenize is not None:
+            # the reference ranks the host copy (ddpm.py:1556); the same values are ranked here on the device, and only
+            # the B selected waveforms are copied out
+            n_total, rows = (Bl, None) if glob is None else (glob[0] * n_gen, glob[1])
+            similarity = self.native_ranker()(wave.reshape(Bl, -1), texts, rows=rows, n_total=n_total)
+            _, best = select_best(np.zeros(Bl), similarity.cpu(), B)
+            return self._egress(wave[best])
         waveform = self._egress(wave)                                                     # ddpm.py:936
         if n_gen > 1:
             if self.ranker is None:
@@ -455,7 +498,7 @@ class NativeAudioLDM2:
 
 def build_model(ckpt_path=None, config=None, device=None, model_name="audioldm2-full", *, synthetic: Optional[bool] = None,
                 cond_provider=None, ranker: Optional[Callable] = None, t5_len: int = 32, ctx_max_len=None, seqgen_index: int = 0,
-                t5_index: Optional[int] = None, **engine_kw):
+                t5_index: Optional[int] = None, clap_tokenize: Optional[Callable] = None, **engine_kw):
     """pipeline.py:142-179.  ``ckpt_path`` is a reference ``<model_name>.pth`` (``["state_dict"]``, key layout of SURVEY.md
     8b); without it (no network here, utils.py:209-219) the seeded synthetic checkpoint is used.  For audioldm2-full / -large
     the AudioMAE generator's weights are taken too (``cond_stage_models.<seqgen_index>.``), for encoder-level providers.  Engines are planned lazily
@@ -467,7 +510,12 @@ def build_model(ckpt_path=None, config=None, device=None, model_name="audioldm2-
     (``cond_stage_models.<t5_index>.model.``, ddpm.py:1529-1533); the *_t5 models use ``cond_stage_models.<t5_index>``
     (default 0) for both.  The CLAP text weights, for token-level ``film_clap_cond1``: the generator's first inner model
     (``cond_stage_models.<seqgen_index>.cond_stage_models.0.model.``) for audioldm2-full / -large,
-    ``cond_stage_models.0.model.`` for audioldm_48k.  Synthetic weights are generated on first token-level use."""
+    ``cond_stage_models.0.model.`` for audioldm_48k.  Synthetic weights are generated on first token-level use.
+    ``clap_tokenize`` (keyword only; the RoBERTa tokenizer, ``texts -> (ids, mask)``): rank the candidates of
+    n_candidate_gen_per_text > 1 natively with the reference's ``clap.model.*`` (its HTSAT audio branch and its text
+    branch; synthetic weights made on first use without a checkpoint).  It excludes ``ranker``."""
+    if ranker is not None and clap_tokenize is not None:
+        raise ValueError("pass either a ranker or clap_tokenize (the native CLAP ranker), not both")
     if device is None or device == "auto":
         device = torch.device("cuda:0")          # the native path has no CPU / MPS fallback
     cfg = arch.model_config(model_name) if config is None else config
@@ -483,6 +531,7 @@ def build_model(ckpt_path=None, config=None, device=None, model_name="audioldm2-
         t5c = synth.t5_state_dict if arch.has_t5(cfg) else None
         t5u = None
         clap = synth.clap_text_state_dict if arch.has_clap(cfg) else None
+        rank = (synth.clap_audio_state_dict, synth.clap_text_state_dict)
         if ctx_max_len is None:
             n_cross = len([c for c in cfg["unet"]["context_dim"] if c is not None])
             ctx_max_len = (8, t5_len) if n_cross > 1 else (t5_len,)
@@ -502,8 +551,12 @@ def build_model(ckpt_path=None, config=None, device=None, model_name="audioldm2-
             clap = model.split_clap_text_state_dict(sd, f"cond_stage_models.{seqgen_index}.cond_stage_models.0.model.")
         elif arch.has_clap(cfg):
             clap = model.split_clap_text_state_dict(sd, "cond_stage_models.0.model.")
+        rank = None
+        if clap_tokenize is not None:
+            rank = (model.split_clap_audio_state_dict(sd, "clap.model."), model.split_clap_text_state_dict(sd, "clap.model."))
     ld = NativeAudioLDM2(cfg, un, vae, voc, device, scale_factor=sf, ctx_max_len=ctx_max_len, seqgen_sd=seq,
-                         t5_sd=t5c, t5_uncond_sd=t5u, clap_sd=clap,
+                         t5_sd=t5c, t5_uncond_sd=t5u, clap_sd=clap, clap_rank_sd=rank if clap_tokenize is not None else None,
+                         clap_tokenize=clap_tokenize,
                          cond_provider=cond_provider or SyntheticConditioning(cfg, t5_len=t5_len, device=device), ranker=ranker,
                          **engine_kw)
     ld.model_name = model_name

@@ -296,6 +296,44 @@ class Plan:
                     setattr(a, name, P(o[name]))
                 for name in ("B", "L", "C", "P"):
                     setattr(a, name, int(o[name]))
+            elif k == "htsat_logmel":
+                op.kind = _lib.OP_HTSAT_LOGMEL
+                a = op.u.htsat_logmel
+                for name in ("wav", "taps", "melW", "bn_mean", "bn_var", "bn_w", "bn_b", "out"):
+                    setattr(a, name, P(o.get(name)))
+                for name in ("n", "L", "up", "L48", "T"):
+                    setattr(a, name, int(o[name]))
+                a.eps = float(o["eps"])
+            elif k == "htsat_patch":
+                op.kind = _lib.OP_HTSAT_PATCH
+                a = op.u.htsat_patch
+                for name in ("mel", "w", "bias", "gamma", "beta", "out"):
+                    setattr(a, name, P(o[name]))
+                a.n, a.T, a.eps = int(o["n"]), int(o["T"]), float(o["eps"])
+            elif k == "htsat_attn":
+                op.kind = _lib.OP_HTSAT_ATTN
+                a = op.u.htsat_attn
+                for name in ("qkv", "bias", "mask", "out_hi", "out_lo"):
+                    setattr(a, name, P(o.get(name)))
+                for name in ("n", "R", "shift", "heads", "head_dim", "C", "ld_qkv", "ldo"):
+                    setattr(a, name, int(o[name]))
+                a.scale = float(o["scale"])
+            elif k == "htsat_merge":
+                op.kind = _lib.OP_HTSAT_MERGE
+                a = op.u.htsat_merge
+                for name in ("x", "gamma", "beta", "out_hi", "out_lo"):
+                    setattr(a, name, P(o.get(name)))
+                for name in ("n", "R", "C", "ldo"):
+                    setattr(a, name, int(o[name]))
+                a.eps = float(o["eps"])
+            elif k == "htsat_head":
+                op.kind = _lib.OP_HTSAT_HEAD
+                a = op.u.htsat_head
+                for name in ("x", "gamma", "beta", "w1_t", "b1", "w2_t", "b2", "out"):
+                    setattr(a, name, P(o[name]))
+                for name in ("n", "ntok", "C", "P"):
+                    setattr(a, name, int(o[name]))
+                a.eps = float(o["eps"])
             elif k == "copy":
                 op.kind = _lib.OP_COPY
                 c = op.u.copy
@@ -1440,5 +1478,291 @@ def build_clap_text(sd: Optional[Dict[str, torch.Tensor]], batch: int, length: i
     P.mark("end")
     assert P.arena.size == 0, "encoder plans reference the shared weight arena only"
     pl = P.finish(io, meta=dict(B=B, L=L, n_layer=W.n_layer))
+    pl.arena = W.arena
+    return pl
+
+
+# ==============================================================================================
+# CLAP audio embedding from the waveform (CLAP.get_audio_embedding, clap/open_clip/model.py:752-777; HTSAT-base,
+# clap/open_clip/htsat.py; the resample and truncation of encoders/modules.py:689-716)
+# ==============================================================================================
+HTSAT_GELU_ROWS = 32768      # rows per clap_gelu launch (its grid's y dimension holds at most 65535)
+
+
+def htsat_resample_taps(orig_freq: int = 16000, new_freq: int = 48000, lowpass_filter_width: int = 6,
+                        rolloff: float = 0.99) -> torch.Tensor:
+    """torchaudio.functional.resample's sinc_interp_hann kernel (functional.py _get_sinc_resample_kernel) for a float32
+    waveform, computed as torchaudio computes it (in float32): [new / gcd, 2 width + orig / gcd] -- [3, 15] for 16 -> 48 kHz.
+    Output sample new * q + j = sum_m taps[j, m] x[orig * q + m - width] (zero padding)."""
+    g = math.gcd(orig_freq, new_freq)
+    orig, new = orig_freq // g, new_freq // g
+    base = min(orig, new) * rolloff
+    width = math.ceil(lowpass_filter_width * orig / base)
+    dt = torch.float32
+    idx = torch.arange(-width, width + orig, dtype=dt)[None, None] / orig
+    t = torch.arange(0, -new, -1, dtype=dt)[:, None, None] / new + idx
+    t *= base
+    t = t.clamp_(-lowpass_filter_width, lowpass_filter_width)
+    window = torch.cos(t * math.pi / lowpass_filter_width / 2) ** 2
+    t *= math.pi
+    k = torch.where(t == 0, torch.tensor(1.0).to(t), t.sin() / t)
+    k *= window * (base / orig)
+    return k[:, 0].contiguous()
+
+
+def htsat_bicubic(T: int, out: int = 1024) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The time-axis weights of F.interpolate(mode="bicubic", align_corners=True) from T to ``out`` frames, in float32 as
+    upsample_bicubic2d computes them (the kernel does the same arithmetic): source x = ((T - 1) / (out - 1)) t, i0 =
+    floor(x), t = x - i0, cubic-convolution weights with A = -0.75.  -> (rows [out, 4] clamped to [0, T), weights [out, 4])."""
+    scale = torch.tensor((T - 1) / 1.0, dtype=torch.float32) / torch.tensor(out - 1, dtype=torch.float32)
+    x = scale * torch.arange(out, dtype=torch.float32)
+    i0 = torch.clamp(torch.floor(x).long(), max=T - 1)
+    t = torch.clamp(x - i0.float(), 0.0, 1.0)
+    A = -0.75
+
+    def c1(v):
+        return ((A + 2.0) * v - (A + 3.0)) * v * v + 1.0
+
+    def c2(v):
+        return ((A * v - 5.0 * A) * v + 8.0 * A) * v - 4.0 * A
+
+    t2 = 1.0 - t
+    w = torch.stack([c2(t + 1.0), c1(t), c1(t2), c2(t2 + 1.0)], 1)
+    rows = (i0[:, None] + torch.arange(-1, 3)[None]).clamp(0, T - 1)
+    return rows, w
+
+
+def htsat_relative_position_index(window: int = 8) -> torch.Tensor:
+    """WindowAttention.relative_position_index (htsat.py:384-401): [w^2, w^2], the row of the [(2w - 1)^2, heads] bias
+    table for query i, key j of a window: (dy + w - 1) (2w - 1) + (dx + w - 1)."""
+    yy, xx = torch.meshgrid(torch.arange(window), torch.arange(window), indexing="ij")
+    c = torch.stack([yy.reshape(-1), xx.reshape(-1)])
+    rel = c[:, :, None] - c[:, None, :] + (window - 1)
+    return rel[0] * (2 * window - 1) + rel[1]
+
+
+def htsat_shift_mask(R: int, window: int = 8, shift: int = 4) -> torch.Tensor:
+    """SwinTransformerBlock.attn_mask (htsat.py:545-576) of a shifted block on an R x R grid: [(R / w)^2, w^2, w^2], 0
+    where query and key come from the same region of the rolled grid, -100 elsewhere."""
+    lab = torch.zeros(R, R)
+    cnt = 0
+    for hs in (slice(0, -window), slice(-window, -shift), slice(-shift, None)):
+        for ws in (slice(0, -window), slice(-window, -shift), slice(-shift, None)):
+            lab[hs, ws] = cnt
+            cnt += 1
+    m = lab.reshape(R // window, window, R // window, window).permute(0, 2, 1, 3).reshape(-1, window * window)
+    d = m[:, None, :] - m[:, :, None]
+    return torch.where(d != 0, torch.tensor(-100.0), torch.tensor(0.0))
+
+
+def htsat_block_shift(R: int, j: int) -> int:
+    """Shift of block j on an R x R grid: window // 2 on odd blocks, 0 where the grid is no larger than a window."""
+    w = arch.CLAP_AUDIO["window"]
+    return 0 if R <= w or j % 2 == 0 else w // 2
+
+
+def htsat_depths(sd: Dict[str, torch.Tensor], prefix: str = "") -> Tuple[int, ...]:
+    """Swin blocks per stage of an audio branch whose keys are ``prefix + "audio_branch.layers.<i>.blocks.<j>.*"``.
+    Raises KeyError when a stage has none."""
+    out = []
+    for i in range(len(arch.CLAP_AUDIO["depths"])):
+        pre = f"{prefix}audio_branch.layers.{i}.blocks."
+        out.append(len({k[len(pre):].split(".")[0] for k in sd if k.startswith(pre)}))
+    if 0 in out:
+        raise KeyError(f"no HTSAT blocks for some stage under {prefix}audio_branch.layers.<i>.blocks. (found {out})")
+    return tuple(out)
+
+
+@dataclass
+class ClapAudioWeights:
+    """The audio branch's weight arena, packed once and shared by the plans of every (n, L, sr); ``bounds``: name ->
+    the largest magnitude a value entering that operand plane can take (clap_audio_plane_bounds)."""
+    arena: torch.Tensor
+    depths: Tuple[int, ...]
+    refs: Dict[str, object]
+    bounds: Dict[str, float]
+
+
+def clap_audio_plane_bounds(sd: Dict[str, torch.Tensor], depths) -> Dict[str, float]:
+    """Bounds, from the weights alone, on every value the encoder writes into fp16 operand planes.  Each is a LayerNorm
+    output y = gamma * z + beta with ||z||_2 <= sqrt(C), a linear function of one, or a convex combination / GELU of those:
+      LayerNorm output (norm1, norm2, downsample.norm)    |y_c| <= |gamma_c| sqrt(C) + |beta_c|
+      v = W_v y + b_v, fc1 pre-activation u = W y + b     |u_n| <= ||w_n * gamma||_2 sqrt(C) + |w_n . beta| + |b_n|
+      attention output                                    a mix of rows of v with weights summing to 1: v's bound
+      GELU output (fc2's operand)                         |gelu(u)| <= |u|
+    name (the reference's module) -> bound, in float64."""
+    d = lambda n: sd[n].double()
+
+    def ln(n):
+        g, b = d(n + ".weight"), d(n + ".bias")
+        return float((g.abs() * math.sqrt(g.numel()) + b.abs()).max())
+
+    def lin(w, b, ln_name):
+        g, be = d(ln_name + ".weight"), d(ln_name + ".bias")
+        return float(((w * g[None]).norm(dim=1) * math.sqrt(g.numel()) + (w @ be).abs() + b.abs()).max())
+
+    out = {}
+    E = arch.CLAP_AUDIO["embed_dim"]
+    for i, depth in enumerate(depths):
+        C = E * 2 ** i
+        for j in range(depth):
+            b = f"audio_branch.layers.{i}.blocks.{j}"
+            out[f"{b}.norm1"] = ln(f"{b}.norm1")
+            out[f"{b}.attn.qkv (v)"] = lin(d(f"{b}.attn.qkv.weight")[2 * C:], d(f"{b}.attn.qkv.bias")[2 * C:], f"{b}.norm1")
+            out[f"{b}.norm2"] = ln(f"{b}.norm2")
+            out[f"{b}.mlp.fc1"] = lin(d(f"{b}.mlp.fc1.weight"), d(f"{b}.mlp.fc1.bias"), f"{b}.norm2")
+        if i < len(depths) - 1:
+            out[f"audio_branch.layers.{i}.downsample.norm"] = ln(f"audio_branch.layers.{i}.downsample.norm")
+    return out
+
+
+def pack_clap_audio_weights(sd: Dict[str, torch.Tensor], **pk) -> ClapAudioWeights:
+    """Weights of model.split_clap_audio_state_dict / synth.clap_audio_state_dict -> arena: the front end (resample taps,
+    melW, bn0), the patch embedding, per block LayerNorm vectors, the qkv / proj / fc1 / fc2 matrices (with biases) as
+    two-plane tile images and the relative-position bias gathered to [heads, 64, 64], per shifted stage the window mask,
+    per PatchMerging its LayerNorm and reduction, and the final LayerNorm and audio_projection in fp32 ([in, out]) for the
+    head kernel.  Raises ValueError, naming the layer, if a value entering an operand plane could exceed the fp16 range
+    (clap_audio_plane_bounds)."""
+    depths = htsat_depths(sd)
+    bounds = clap_audio_plane_bounds(sd, depths)
+    for name, v in bounds.items():
+        if not v <= FP16_MAX:
+            raise ValueError(f"CLAP audio branch: values entering the fp16 operand planes after {name} can reach {v:.6g}, "
+                             f"beyond the fp16 range ({FP16_MAX:g}); these weights cannot be encoded without clamping")
+    A = arch.CLAP_AUDIO
+    P = Planner(**pk)
+
+    def lin(n, bias=True) -> WMat:
+        wm, taps, cp = packing.conv_weight_matrix(sd[n + ".weight"].float())
+        return P.wmat(wm, sd[n + ".bias"].float() if bias else None, taps, cp, bn=CLAP_BN)
+
+    a = "audio_branch"
+    vec2 = lambda n: (P.vec(sd[n + ".weight"]), P.vec(sd[n + ".bias"]))
+    rpi = htsat_relative_position_index(A["window"]).reshape(-1)
+    r: Dict[str, object] = {
+        "taps": P.vec(htsat_resample_taps()),
+        "melW": P.vec(sd[f"{a}.logmel_extractor.melW"]),
+        "bn": tuple(P.vec(sd[f"{a}.bn0.{k}"]) for k in ("running_mean", "running_var", "weight", "bias")),
+        "patch_w": P.vec(sd[f"{a}.patch_embed.proj.weight"].reshape(A["embed_dim"], -1)),
+        "patch_b": P.vec(sd[f"{a}.patch_embed.proj.bias"]),
+        "patch_ln": vec2(f"{a}.patch_embed.norm"),
+        "norm": vec2(f"{a}.norm"),
+        "w1_t": P.vec(sd["audio_projection.0.weight"].float().t()), "b1": P.vec(sd["audio_projection.0.bias"]),
+        "w2_t": P.vec(sd["audio_projection.2.weight"].float().t()), "b2": P.vec(sd["audio_projection.2.bias"]),
+    }
+    R = A["spec_size"] // A["patch"]
+    for i, depth in enumerate(depths):
+        if R > A["window"]:
+            r[f"{i}.mask"] = P.vec(htsat_shift_mask(R, A["window"], A["window"] // 2))
+        for j in range(depth):
+            b = f"{a}.layers.{i}.blocks.{j}"
+            tab = sd[f"{b}.attn.relative_position_bias_table"].float()
+            r[f"{i}.{j}.bias"] = P.vec(tab[rpi].reshape(A["window"] ** 2, A["window"] ** 2, -1).permute(2, 0, 1))
+            r[f"{i}.{j}.ln1"] = vec2(f"{b}.norm1")
+            r[f"{i}.{j}.qkv"] = lin(f"{b}.attn.qkv")
+            r[f"{i}.{j}.proj"] = lin(f"{b}.attn.proj")
+            r[f"{i}.{j}.ln2"] = vec2(f"{b}.norm2")
+            r[f"{i}.{j}.fc1"] = lin(f"{b}.mlp.fc1")
+            r[f"{i}.{j}.fc2"] = lin(f"{b}.mlp.fc2")
+        if i < len(depths) - 1:
+            r[f"{i}.merge_ln"] = vec2(f"{a}.layers.{i}.downsample.norm")
+            r[f"{i}.reduction"] = lin(f"{a}.layers.{i}.downsample.reduction", bias=False)
+        R //= 2
+    return ClapAudioWeights(P.arena.build(), depths, r, bounds)
+
+
+def build_clap_audio(sd: Optional[Dict[str, torch.Tensor]], n: int, length: int, sampling_rate: int,
+                     weights: Optional[ClapAudioWeights] = None, **pk) -> Plan:
+    """CLAP.get_audio_embedding of n clips of ``length`` samples at ``sampling_rate`` (16 000: resampled to 48 kHz on the
+    fly; 48 000), truncated to 480 000 samples at 48 kHz, in fp32.
+
+    io: wav [n, L] fp32 in; embed [n, 512] fp32 out.  Launches: the log-mel front end, the patch embedding, per Swin block
+    LN1, the QKV GEMM, window attention, the proj GEMM + residual, LN2, the fc1 GEMM, erf-GELU (one launch per 32768 rows),
+    the fc2 GEMM + residual; per PatchMerging its gather + LayerNorm and the reduction GEMM; the head.  Marks "begin",
+    "end".  The plan references the arena of ``weights`` (packed from ``sd`` when None)."""
+    W = weights if weights is not None else pack_clap_audio_weights(sd, **pk)
+    A = arch.CLAP_AUDIO
+    n, L, sr = int(n), int(length), int(sampling_rate)
+    if sr not in (16000, 48000):
+        raise ValueError(f"clap audio: sampling rate {sr} (16000 or 48000)")
+    up = 48000 // sr
+    L48 = min(up * L, A["max_samples"])
+    if n < 1 or L48 <= A["n_fft"] // 2:
+        raise ValueError(f"clap audio: {n} clips of {L} samples at {sr} Hz: the 48 kHz signal needs more than "
+                         f"{A['n_fft'] // 2} samples (reflect padding)")
+    T = L48 // A["hop"] + 1
+    P = Planner(**pk)
+    r = W.refs
+    E, Hd, win, eps = A["embed_dim"], A["head_dim"], A["window"], A["eps"]
+    wav = P.raw(n * L * 4)
+    embed = P.raw(n * A["joint_dim"] * 4)
+    io = dict(wav=("f32", wav, (n, L)), embed=("f32", embed, (n, A["joint_dim"])))
+
+    P.mark("begin")
+    P.tag = 0
+    mel = P.raw(n * T * A["n_mels"] * 4)
+    bm, bv, bw, bb = r["bn"]
+    P.ops.append(dict(kind="htsat_logmel", tag=0, wav=wav, taps=r["taps"] if up == 3 else None, melW=r["melW"], bn_mean=bm,
+                      bn_var=bv, bn_w=bw, bn_b=bb, out=mel, n=n, L=L, up=up, L48=L48, T=T, eps=A["bn_eps"]))
+    R = A["spec_size"] // A["patch"]
+    x = P.f32(n * R * R, E)
+    P.ops.append(dict(kind="htsat_patch", tag=0, mel=mel, w=r["patch_w"], bias=r["patch_b"], gamma=r["patch_ln"][0],
+                      beta=r["patch_ln"][1], out=x.ref, n=n, T=T, eps=eps))
+    P.free(mel)
+    blk = 0
+    for i, depth in enumerate(W.depths):
+        C, H = E * 2 ** i, A["heads"][i]
+        rows = n * R * R
+        for j in range(depth):
+            blk += 1
+            P.tag = blk
+            shift = htsat_block_shift(R, j)
+            # x = x + proj(WindowAttention(norm1(x)))
+            a = P.prep(_lib.PREP_LN, x, None, *r[f"{i}.{j}.ln1"], eps=eps)
+            qkv = P.f32(rows, 3 * C)
+            P.gemm(a, r[f"{i}.{j}.qkv"], B=1, H=rows, out=qkv)
+            P.free(a)
+            o = P.planes(rows, C)
+            P.ops.append(dict(kind="htsat_attn", tag=P.tag, qkv=qkv.ref, bias=r[f"{i}.{j}.bias"],
+                              mask=r[f"{i}.mask"] if shift else None, out_hi=o.hi, out_lo=o.lo, n=n, R=R, shift=shift,
+                              heads=H, head_dim=Hd, C=C, ld_qkv=3 * C, ldo=o.Cp, scale=Hd ** -0.5))
+            P.free(qkv)
+            y = P.f32(rows, C)
+            P.gemm(o, r[f"{i}.{j}.proj"], B=1, H=rows, out=y, res=x)
+            P.free(o, x)
+            x = y
+            # x = x + fc2(gelu(fc1(norm2(x))))
+            a = P.prep(_lib.PREP_LN, x, None, *r[f"{i}.{j}.ln2"], eps=eps)
+            Fd = A["mlp_ratio"] * C
+            hm = P.f32(rows, Fd)
+            P.gemm(a, r[f"{i}.{j}.fc1"], B=1, H=rows, out=hm)
+            P.free(a)
+            g = P.planes(rows, Fd)
+            for r0 in range(0, rows, HTSAT_GELU_ROWS):
+                nr = min(HTSAT_GELU_ROWS, rows - r0)
+                P.ops.append(dict(kind="clap_gelu", tag=P.tag, x=hm.ref + r0 * Fd * 4, out_hi=g.hi + r0 * g.Cp * 2,
+                                  out_lo=g.lo + r0 * g.Cp * 2, rows=nr, F=Fd, ld_x=Fd, ldo=g.Cp))
+            P.free(hm)
+            y = P.f32(rows, C)
+            P.gemm(g, r[f"{i}.{j}.fc2"], B=1, H=rows, out=y, res=x)
+            P.free(g, x)
+            x = y
+        if i < len(W.depths) - 1:
+            m = P.planes(rows // 4, 4 * C)
+            P.ops.append(dict(kind="htsat_merge", tag=P.tag, x=x.ref, gamma=r[f"{i}.merge_ln"][0], beta=r[f"{i}.merge_ln"][1],
+                              out_hi=m.hi, out_lo=m.lo, n=n, R=R, C=C, ldo=m.Cp, eps=eps))
+            P.free(x)
+            x = P.f32(rows // 4, 2 * C)
+            P.gemm(m, r[f"{i}.reduction"], B=1, H=rows // 4, out=x)
+            P.free(m)
+            R //= 2
+    P.tag = blk + 1
+    Cf = x.C
+    P.ops.append(dict(kind="htsat_head", tag=P.tag, x=x.ref, gamma=r["norm"][0], beta=r["norm"][1], w1_t=r["w1_t"],
+                      b1=r["b1"], w2_t=r["w2_t"], b2=r["b2"], out=embed, n=n, ntok=R * R, C=Cf, P=A["joint_dim"], eps=eps))
+    P.free(x)
+    P.mark("end")
+    assert P.arena.size == 0, "encoder plans reference the shared weight arena only"
+    pl = P.finish(io, meta=dict(n=n, L=L, sr=sr, T=T, depths=W.depths))
     pl.arena = W.arena
     return pl

@@ -224,3 +224,62 @@ def conditioning(cfg: dict, batch: int, seed: int = 77, t5_len: int = 32, device
         cond["y"] = y.to(device)
         unc["y"] = torch.zeros(batch, fd).to(device)
     return cond, unc
+
+
+def clap_audio_state_dict(seed: int = 1240, depths=(2, 2, 12, 2)) -> Dict[str, torch.Tensor]:
+    """Seeded CLAP audio branch (``audio_branch.`` + ``audio_projection``, arch.clap_audio_param_shapes).  torchlibrosa's
+    fixed tensors are made exactly: the STFT weights are the periodic-Hann DFT basis (model.htsat_dft_basis) and melW the
+    Slaney mel filterbank of 48 kHz / 1024 / 64 bins / 50 Hz - 14 kHz.  bn0's running statistics (mean -15 dB, std 15 dB)
+    bring the log-mel of vocoder-like audio (|x| ~ 0.1) to O(1).  Matrices are N(0, 1 / fan_in), with the residual branch
+    outputs (attn.proj, mlp.fc2) at half that gain so that the pre-LN residual stream stays O(1) over 18 blocks; the
+    relative-position tables 0.5 N(0, 1) (a visible bias next to logits of a few units); biases and LayerNorm offsets
+    0.1 N(0, 1), LayerNorm and bn0 weights 1 + 0.1 N(0, 1)."""
+    from . import frontend, model
+    shapes = arch.clap_audio_param_shapes(tuple(depths))
+    g = torch.Generator(device="cpu")
+    g.manual_seed(seed)
+    out = {}
+    for name in sorted(shapes):
+        shp = shapes[name]
+        t = torch.randn(shp, generator=g)
+        if "spectrogram_extractor" in name or "logmel_extractor" in name:
+            continue
+        if name.endswith("running_mean"):
+            t = -15.0 + 0.5 * t
+        elif name.endswith("running_var"):
+            t = 225.0 * (1.0 + 0.05 * t.abs())
+        elif name.endswith("relative_position_bias_table"):
+            t = 0.5 * t
+        elif name.endswith(("norm.weight", "norm1.weight", "norm2.weight", "bn0.weight")):
+            t = 1.0 + 0.1 * t
+        elif len(shp) == 1:
+            t = 0.1 * t
+        else:
+            fan_in = math.prod(shp[1:])
+            t = t / math.sqrt(fan_in) * (0.5 if name.endswith(("attn.proj.weight", "mlp.fc2.weight")) else 1.0)
+        out[name] = t.contiguous()
+    real, imag = model.htsat_dft_basis(arch.CLAP_AUDIO["n_fft"])
+    out["audio_branch.spectrogram_extractor.stft.conv_real.weight"] = real.float()
+    out["audio_branch.spectrogram_extractor.stft.conv_imag.weight"] = imag.float()
+    A = arch.CLAP_AUDIO
+    out["audio_branch.logmel_extractor.melW"] = frontend.mel_basis(A["sample_rate"], A["n_fft"], A["n_mels"], A["fmin"],
+                                                                   A["fmax"]).t().contiguous()
+    return out
+
+
+def clap_tokenize(texts, seed: int = 82, L: int = 512):
+    """A seeded stand-in for the RoBERTa tokenizer (padding="max_length", max_length 512): each text maps
+    deterministically (crc32 of its UTF-8 bytes and the seed, not Python's salted hash) to BOS, 1 .. 30 ids from
+    [3, vocab), EOS, then pad; "" gives [BOS, EOS] as the real tokenizer does.  -> (ids [n, L] int64, mask [n, L] float)."""
+    import zlib
+    A = arch.CLAP_TEXT
+    ids = torch.full((len(texts), L), A["pad_id"], dtype=torch.int64)
+    mask = torch.zeros(len(texts), L)
+    for i, t in enumerate(texts):
+        h = zlib.crc32(t.encode("utf-8")) ^ (seed * 0x9E3779B1 & 0xFFFFFFFF)
+        g = torch.Generator().manual_seed(h)
+        n = 0 if t == "" else 1 + int(torch.randint(30, (1,), generator=g))
+        row = [A["bos_id"]] + torch.randint(3, A["vocab"], (n,), generator=g).tolist() + [A["eos_id"]]
+        ids[i, :len(row)] = torch.tensor(row)
+        mask[i, :len(row)] = 1
+    return ids, mask

@@ -33,6 +33,9 @@
  *   CLAP.get_text_embedding (RoBERTa text branch, pooler,         aldm_program_run(clap program: embedding + LN +
  *       text_projection, F.normalize) clap/open_clip/model.py:     12 blocks + head; ALDM_OP_CLAP_EMBED ..
  *       656-663,730-750; encoders/modules.py:660-735               ALDM_OP_CLAP_HEAD)
+ *   CLAP.get_audio_embedding (HTSAT-base audio branch,             aldm_program_run(clap audio program: log-mel, patch
+ *       audio_projection, F.normalize) clap/open_clip/htsat.py,    embedding, 18 Swin blocks, 3 merges, head;
+ *       model.py:752-777; encoders/modules.py:689-716              ALDM_OP_HTSAT_LOGMEL .. ALDM_OP_HTSAT_HEAD)
  *
  * Conventions
  *   - all pointers are DEVICE pointers unless named host_*; buffers are caller-owned (torch
@@ -56,7 +59,7 @@
 extern "C" {
 #endif
 
-#define ALDM_ABI_VERSION 11
+#define ALDM_ABI_VERSION 12
 #define ALDM_MAX_TAPS 16
 
 enum {
@@ -397,13 +400,85 @@ typedef struct aldm_clap_head_desc {
 } aldm_clap_head_desc;
 int aldm_clap_head(const aldm_clap_head_desc* d, void* stream);
 
+/* ---- CLAP HTSAT-base audio branch (csrc/audio/htsat.cu) -----------------------------------------
+ * Pre-LN Swin transformer over a 64 x 64 patch grid (stages of 64, 32, 16 and 8): the residual stream is fp32 [n * R * R, C]
+ * in natural token order (row-major over the grid); every projection is a two-plane GEMM. */
+
+/* Log-mel front end, one frame per CTA: the 48 kHz signal (up = 1: wav itself; up = 3: torchaudio's 16 -> 48 kHz resample
+ * with taps [3][15], sample 3q + j = sum_m taps[j][m] wav[q + m - 7], zeros outside), truncated to L48 = min(up L, 480000)
+ * samples, reflect-centred frames of 1024 every 480 (T = L48 / 480 + 1), periodic Hann, power spectrum, power @ melW
+ * [513, 64], 10 log10(max(., 1e-10)), then BatchNorm with running statistics.  L48 <= 512 (no reflect padding) is
+ * ALDM_E_SHAPE; up other than 1 or 3 is ALDM_E_UNSUPPORTED. */
+typedef struct aldm_htsat_logmel_desc {
+  const float* wav;          /* [n, L] */
+  const float* taps;         /* [3, 15] (up = 3), else unused */
+  const float* melW;         /* [513, 64] */
+  const float* bn_mean; const float* bn_var; const float* bn_w; const float* bn_b;   /* [64] */
+  float* out;                /* [n, T, 64] */
+  int32_t n, L, up, L48, T;
+  float eps;
+} aldm_htsat_logmel_desc;
+int aldm_htsat_logmel(const aldm_htsat_logmel_desc* d, void* stream);
+
+/* reshape_wav2img + patch embedding: bicubic (align_corners, A = -0.75) interpolation of the T frames to 1024, the fold
+ * image[chunk * 64 + mel, t - 256 chunk], Conv2d(1, 128, 4, stride 4) with bias (w [128, 16] in (dy, dx) order) and
+ * LayerNorm(128).  out: the fp32 residual stream [n * 4096, 128].  2 <= T <= 1024. */
+typedef struct aldm_htsat_patch_desc {
+  const float* mel;          /* [n, T, 64] */
+  const float* w; const float* bias;      /* [128, 16], [128] */
+  const float* gamma; const float* beta;  /* [128] */
+  float* out;
+  int32_t n, T;
+  float eps;
+} aldm_htsat_patch_desc;
+int aldm_htsat_patch(const aldm_htsat_patch_desc* d, void* stream);
+
+/* (Shifted) window attention over 8 x 8 windows of an R x R grid rolled by -shift: s = (scale q) . k + bias[h, i, j]
+ * (+ mask[w, i, j] when shift > 0), fp32 softmax and P V.  qkv [n * R * R, ld_qkv] holds q | k | v at columns [0, C),
+ * [C, 2C), [2C, 3C) in natural token order; the output planes [n * R * R, ldo] are written at the same (un-rolled) tokens.
+ * head_dim other than 32 is ALDM_E_UNSUPPORTED; R not a multiple of 8, or shift > 0 without a mask, is ALDM_E_SHAPE. */
+typedef struct aldm_htsat_attn_desc {
+  const float* qkv;
+  const float* bias;         /* [heads, 64, 64] */
+  const float* mask;         /* [(R / 8)^2, 64, 64] (0 / -100), or null when shift = 0 */
+  void* out_hi; void* out_lo;
+  int32_t n, R, shift, heads, head_dim, C, ld_qkv, ldo;
+  float scale;
+} aldm_htsat_attn_desc;
+int aldm_htsat_window_attention(const aldm_htsat_attn_desc* d, void* stream);
+
+/* PatchMerging's gather and norm: row (a, b) of the R/2 x R/2 grid is cat(x(2a, 2b), x(2a+1, 2b), x(2a, 2b+1),
+ * x(2a+1, 2b+1)) [4C], LayerNorm(4C) -> operand planes [n * (R/2)^2, ldo].  C is 128, 256 or 512. */
+typedef struct aldm_htsat_merge_desc {
+  const float* x;            /* [n * R * R, C] */
+  const float* gamma; const float* beta;  /* [4C] */
+  void* out_hi; void* out_lo;
+  int32_t n, R, C, ldo;
+  float eps;
+} aldm_htsat_merge_desc;
+int aldm_htsat_merge(const aldm_htsat_merge_desc* d, void* stream);
+
+/* Per clip, fp32: m = mean over the ntok tokens of LayerNorm(x), t = relu(W1 m + b1), y = W2 t + b2,
+ * out = y / max(||y||_2, 1e-12).  Weights transposed ([in, out]).  C, P <= 1024. */
+typedef struct aldm_htsat_head_desc {
+  const float* x;            /* [n * ntok, C] */
+  const float* gamma; const float* beta;  /* [C] */
+  const float* w1_t; const float* b1;     /* [C, P], [P] */
+  const float* w2_t; const float* b2;     /* [P, P], [P] */
+  float* out;                /* [n, P] */
+  int32_t n, ntok, C, P;
+  float eps;
+} aldm_htsat_head_desc;
+int aldm_htsat_head(const aldm_htsat_head_desc* d, void* stream);
+
 /* ---- programs: flat op tables replayed on a stream / as a CUDA graph ---------------------- */
 
 enum { ALDM_OP_GEMM = 1, ALDM_OP_PREP = 2, ALDM_OP_ATTN = 3, ALDM_OP_SOFTMAX = 4, ALDM_OP_TEMB = 5,
        ALDM_OP_TRANSPOSE = 6, ALDM_OP_PACKB = 7, ALDM_OP_COPY = 8, ALDM_OP_SEQ_ASSEMBLE = 9, ALDM_OP_KV_ATTN = 10,
        ALDM_OP_SEQ_FEEDBACK = 11, ALDM_OP_T5_EMBED = 12, ALDM_OP_T5_RMSNORM = 13, ALDM_OP_T5_ATTN = 14,
        ALDM_OP_T5_GATE = 15, ALDM_OP_CLAP_EMBED = 16, ALDM_OP_CLAP_LN = 17, ALDM_OP_CLAP_ATTN = 18,
-       ALDM_OP_CLAP_GELU = 19, ALDM_OP_CLAP_HEAD = 20 };
+       ALDM_OP_CLAP_GELU = 19, ALDM_OP_CLAP_HEAD = 20, ALDM_OP_HTSAT_LOGMEL = 21, ALDM_OP_HTSAT_PATCH = 22,
+       ALDM_OP_HTSAT_ATTN = 23, ALDM_OP_HTSAT_MERGE = 24, ALDM_OP_HTSAT_HEAD = 25 };
 
 typedef struct aldm_op {
   int32_t kind;
@@ -429,6 +504,11 @@ typedef struct aldm_op {
     aldm_clap_attn_desc clap_attn;
     aldm_clap_gelu_desc clap_gelu;
     aldm_clap_head_desc clap_head;
+    aldm_htsat_logmel_desc htsat_logmel;
+    aldm_htsat_patch_desc htsat_patch;
+    aldm_htsat_attn_desc htsat_attn;
+    aldm_htsat_merge_desc htsat_merge;
+    aldm_htsat_head_desc htsat_head;
   } u;
 } aldm_op;
 
