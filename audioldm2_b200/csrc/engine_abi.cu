@@ -222,6 +222,32 @@ extern "C" int aldm_engine_ddim_step(aldm_engine* e, const float* x, int64_t t, 
   return ALDM_OK;
 }
 
+extern "C" int aldm_engine_plms_step(aldm_engine* e, const float* x_in, int64_t t, const float* x_base, const float* held1,
+                                     const float* held2, const float* held3, int32_t order, float* e_t_out, float a_t,
+                                     float a_prev, float sqrt_one_minus_at, float guidance, float* x_prev, float* pred_x0,
+                                     void* stream) {
+  ALDM_REQUIRE(e && x_in && x_base && x_prev, ALDM_E_ARG, "plms_step: null argument");
+  ALDM_REQUIRE(x_prev != x_base, ALDM_E_ARG, "plms_step: x_prev must not alias x_base");
+  // the per-lane kernel checks order and held slots too, but only after the UNet has run: check them before
+  ALDM_REQUIRE(order >= ALDM_PLMS_AVERAGE && order <= 4, ALDM_E_ARG, "plms_step: order=%d", order);
+  ALDM_REQUIRE(((order != ALDM_PLMS_AVERAGE && order < 2) || held1) && (order < 3 || held2) && (order < 4 || held3),
+               ALDM_E_ARG, "plms_step: order %d without the held values it needs", order);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int rc = run_unet(e, x_in, t, st);
+  if (rc) return rc;
+  const aldm_engine_desc& d = e->d;
+  const long long n = (long long)(d.B / d.n_lanes) * d.latent_elems;
+  auto at = [&](const float* p, int l) { return p ? p + l * n : nullptr; };
+  for (int l = 0; l < d.n_lanes; ++l) {
+    const float* eps = d.lane[l].eps_slot;
+    rc = aldm_plms_step(x_base + l * n, eps, eps + n, at(held1, l), at(held2, l), at(held3, l), order,
+                        e_t_out ? e_t_out + l * n : nullptr, x_prev + l * n, pred_x0 ? pred_x0 + l * n : nullptr, n, a_t,
+                        a_prev, sqrt_one_minus_at, guidance, stream);
+    if (rc) return rc;
+  }
+  return ALDM_OK;
+}
+
 extern "C" int aldm_engine_vae_decode(aldm_engine* e, const float* z, float* mel, void* stream) {
   ALDM_REQUIRE(e && z && e->d.vae_dec, ALDM_E_ARG, "vae_decode: engine has no decoder program / null z");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);

@@ -9,7 +9,8 @@ pipeline read like the reference:
     encode_first_stage(x) (+ posterior)      ddpm.py:941-943, 793-802
     q_sample / masked blend                  ddpm.py:430-436, ddim.py:226-231
 
-plus ``p_sample_ddim`` (ddim.py:265-355) fused into one native step.  Conditioning is either the
+plus ``p_sample_ddim`` (ddim.py:265-355) fused into one native step, and each UNet evaluation of ``p_sample_plms``
+(plms.py:260-360) with its update as one native step.  Conditioning is either the
 reference's keyed cond-dict (``{"film_clap_...": y, "crossattn_...": [ctx, mask], ...}``, unpacked by
 ``unpack_cond_dict`` exactly as DiffusionWrapper.forward does) or the already-unpacked
 ``{"context_list": [...], "mask_list": [...], "y": ...}``.
@@ -29,7 +30,7 @@ import numpy as np
 import torch
 
 from . import _lib, arch, engine, plan
-from .sampler import DDIMSampler, ddpm_tables
+from .sampler import DDIMSampler, PLMSSampler, ddpm_tables
 
 
 def split_state_dict(state_dict: Dict[str, torch.Tensor]):
@@ -359,6 +360,24 @@ class NativeLatentDiffusion:
             self._st()), "engine_ddim_step")
         return out
 
+    def p_sample_plms(self, x_in, t: int, x_base, held: Sequence[torch.Tensor], order: int, st: dict, guidance: float,
+                      e_t_out=None, out=None, pred_x0=None):
+        """One get_model_output + get_x_prev_and_pred_x0 of plms.py:281-358: eps_u/eps_c at (x_in, t), e_t = e_u + s (e_c -
+        e_u), e' of ``order`` (1-4, or _lib.PLMS_AVERAGE with held = [the first evaluation's e_t]) over ``held`` (most
+        recent first), x_prev from ``x_base`` with the step's coefficients ``st`` -- one graph replay + the PLMS kernel.
+        ``e_t_out`` receives e_t.  ``out`` may be ``x_in`` but not ``x_base``."""
+        out = torch.empty_like(x_base) if out is None else out
+        bufs = [x_in, x_base, out] + list(held) + [b for b in (e_t_out, pred_x0) if b is not None]
+        assert all(b.is_contiguous() and b.dtype == torch.float32 and b.shape == x_base.shape for b in bufs)
+        assert x_base.shape[0] == self.batch and len(held) <= 3
+        h = [b.data_ptr() for b in held] + [None] * (3 - len(held))
+        _lib.check(_lib.lib().aldm_engine_plms_step(
+            self._engine, x_in.data_ptr(), int(t), x_base.data_ptr(), *h, int(order),
+            e_t_out.data_ptr() if e_t_out is not None else None, st["a_t"], st["a_prev"], st["sqrt_one_minus_at"],
+            float(guidance), out.data_ptr(), pred_x0.data_ptr() if pred_x0 is not None else None, self._st()),
+            "engine_plms_step")
+        return out
+
     def masked_blend(self, img, x0, mask, q_noise, st: dict):
         return engine.masked_blend(img, x0, mask, q_noise, st["sqrt_acp_t"], st["sqrt_1m_acp_t"])
 
@@ -400,8 +419,9 @@ class NativeLatentDiffusion:
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
     def generate_latent(self, cond: dict, uncond: Optional[dict], ddim_steps: int = 200, guidance: float = 3.5, eta: float = 1.0,
-                        x_T=None, noise_fn=None, mask=None, x0=None):
-        sampler = DDIMSampler(self)
+                        x_T=None, noise_fn=None, mask=None, x0=None, use_plms: bool = False):
+        """sample_log (ddpm.py:1449-1461): DDIM, or PLMS with ``use_plms`` (``eta`` then ignored, as the reference does)."""
+        sampler = PLMSSampler(self) if use_plms else DDIMSampler(self)
         z, _ = sampler.sample(S=ddim_steps, batch_size=self.batch, shape=self.latent, conditioning=cond, eta=eta,
                               unconditional_guidance_scale=guidance, unconditional_conditioning=uncond, x_T=x_T,
                               noise_fn=noise_fn, mask=mask, x0=x0)
@@ -409,8 +429,8 @@ class NativeLatentDiffusion:
 
     @torch.no_grad()
     def generate_waveform(self, cond: dict, uncond: Optional[dict], ddim_steps: int = 200, guidance: float = 3.5, eta: float = 1.0,
-                          x_T=None, noise_fn=None, mask=None, x0=None):
-        z = self.generate_latent(cond, uncond, ddim_steps, guidance, eta, x_T, noise_fn, mask, x0)
+                          x_T=None, noise_fn=None, mask=None, x0=None, use_plms: bool = False):
+        z = self.generate_latent(cond, uncond, ddim_steps, guidance, eta, x_T, noise_fn, mask, x0, use_plms)
         mel = self.decode_first_stage(z)
         return self.mel_spectrogram_to_waveform(mel)
 

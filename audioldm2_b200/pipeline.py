@@ -424,13 +424,14 @@ class NativeAudioLDM2:
                               unconditional_conditioning, use_plms, time_mask_ratio_start_and_end, freq_mask_ratio_start_and_end)
 
     def _generate(self, batch, ddim_steps, ddim_eta, x_T, n_gen, guidance, uncond, use_plms, tmask, fmask):
-        assert x_T is None and not use_plms, "the native path implements the DDIM sampler (pipeline.py never asks for PLMS)"
+        """sample_log (ddpm.py:1449-1461): DDIMSampler, or PLMSSampler with ``use_plms`` (which ignores ``ddim_eta``)."""
+        assert x_T is None, "the native path draws x_T itself, as pipeline.py's calls do"
         shard = parallel.current_shard(len(batch["text"]))
         if shard is not None:              # one process per GPU: this rank generates prompts [lo, hi) of the call (SURVEY.md 8e)
-            return self._generate_sharded(shard, batch, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask)
-        return self._generate_local(batch, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, None)
+            return self._generate_sharded(shard, batch, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, use_plms)
+        return self._generate_local(batch, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, None, use_plms=use_plms)
 
-    def _generate_sharded(self, shard, batch, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask):
+    def _generate_sharded(self, shard, batch, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, use_plms=False):
         """Every rank runs the same call with the same seed; prompts are cut into contiguous shards, the noise of the
         single-process latent batch (rows i + k * B) is drawn in full on every rank and sliced, and the selected waveforms are
         all-gathered at the end.  Results equal the single-process call row for row."""
@@ -440,11 +441,12 @@ class NativeAudioLDM2:
         rows = [i + k * B for k in range(n_gen) for i in range(lo, hi)]
         # conditioning of the whole call, this rank's rows: made by _generate_local after the posterior draw, as in one process
         cond_l = lambda: self._sharded_conditioning(batch, lo, hi)
-        out = self._generate_local(local, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, (B, rows), cond_l)
+        out = self._generate_local(local, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, (B, rows), cond_l, use_plms)
         full = parallel.all_gather_rows(torch.from_numpy(out).to(self.device), B)
         return self._egress(full)
 
-    def _generate_local(self, batch, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, glob, cond_rows=None):
+    def _generate_local(self, batch, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, glob, cond_rows=None,
+                        use_plms=False):
         masked = tmask is not None
         B = len(batch["text"])
         Bl = B * n_gen
@@ -477,7 +479,7 @@ class NativeAudioLDM2:
             uncond = self.unconditioning(Bl, uncond)                                      # ddpm.py:1529-1536
         texts = list(batch["text"]) * n_gen
         wave = eng.generate_waveform(cond, uncond, ddim_steps=ddim_steps, guidance=guidance, eta=ddim_eta, mask=mask, x0=x0,
-                                     x_T=x_T, noise_fn=noise_fn)
+                                     x_T=x_T, noise_fn=noise_fn, use_plms=use_plms)
         if n_gen > 1 and self.clap_tokenize is not None:
             # the reference ranks the host copy (ddpm.py:1556); the same values are ranked here on the device, and only
             # the B selected waveforms are copied out
@@ -582,14 +584,15 @@ def make_batch_for_text_to_audio(text, transcription="", waveform=None, fbank=No
 
 
 def text_to_audio(latent_diffusion, text, transcription="", seed=42, ddim_steps=200, duration=10, batchsize=1,
-                  guidance_scale=3.5, n_candidate_gen_per_text=3, latent_t_per_second=25.6, config=None):
-    """pipeline.py:181-211 -> np.ndarray [batchsize, 1, samples] float32 in (-1, 1)."""
+                  guidance_scale=3.5, n_candidate_gen_per_text=3, latent_t_per_second=25.6, config=None, *, use_plms=False):
+    """pipeline.py:181-211 -> np.ndarray [batchsize, 1, samples] float32 in (-1, 1).  ``use_plms`` (keyword only) samples
+    with PLMS, as generate_batch(use_plms=True) does: ``ddim_steps`` PLMS steps cost ``ddim_steps`` + 1 UNet pairs."""
     seed_everything(int(seed))
     batch = make_batch_for_text_to_audio(text, transcription=transcription, waveform=None, batchsize=batchsize)
     latent_diffusion.latent_t_size = int(duration * latent_t_per_second)
     with torch.no_grad():
         waveform = latent_diffusion.generate_batch(batch, unconditional_guidance_scale=guidance_scale, ddim_steps=ddim_steps,
-                                                   n_gen=n_candidate_gen_per_text, duration=duration)
+                                                   n_gen=n_candidate_gen_per_text, duration=duration, use_plms=use_plms)
     return waveform
 
 
@@ -613,9 +616,10 @@ def wav_to_fbank(latent_diffusion, original_audio_file_path=None, target_length=
 def super_resolution_and_inpainting(latent_diffusion, text, transcription="", original_audio_file_path=None, seed=42,
                                     ddim_steps=200, duration=None, batchsize=1, guidance_scale=2.5, n_candidate_gen_per_text=3,
                                     time_mask_ratio_start_and_end=(0.40, 0.6), freq_mask_ratio_start_and_end=(1.0, 1.0),
-                                    latent_t_per_second=25.6, config=None, *, waveform=None, waveform_sr=None):
+                                    latent_t_per_second=25.6, config=None, *, waveform=None, waveform_sr=None, use_plms=False):
     """pipeline.py:213-267: STFT/mel front end (K9) -> VAE encoder -> masked DDIM -> decode -> vocoder.  ``waveform`` (+
-    ``waveform_sr``) replaces the file read for callers that already hold the samples."""
+    ``waveform_sr``) replaces the file read for callers that already hold the samples; ``use_plms`` samples with masked
+    PLMS instead (generate_batch_masked(use_plms=True))."""
     seed_everything(int(seed))
     if duration is None:
         duration = latent_diffusion.cfg["latent"][1] / latent_diffusion.cfg["latent_t_per_second"] if waveform is None \
@@ -630,5 +634,5 @@ def super_resolution_and_inpainting(latent_diffusion, text, transcription="", or
         waveform_out = latent_diffusion.generate_batch_masked(
             batch, unconditional_guidance_scale=guidance_scale, ddim_steps=ddim_steps, n_gen=n_candidate_gen_per_text,
             duration=duration, time_mask_ratio_start_and_end=time_mask_ratio_start_and_end,
-            freq_mask_ratio_start_and_end=freq_mask_ratio_start_and_end)
+            freq_mask_ratio_start_and_end=freq_mask_ratio_start_and_end, use_plms=use_plms)
     return waveform_out

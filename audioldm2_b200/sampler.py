@@ -1,6 +1,7 @@
-"""Host-side DDIM scheduler: mirrors ``DDIMSampler`` (latent_diffusion/models/ddim.py) -- the Python
-loop, the schedule tables and the RNG draw order stay on the host exactly as in the reference;
-each loop body (two UNet evaluations + CFG combine + x_{t-1} update) is one native call.
+"""Host-side DDIM and PLMS schedulers: mirror ``DDIMSampler`` (latent_diffusion/models/ddim.py) and ``PLMSSampler``
+(latent_diffusion/models/plms.py) -- the Python loop, the schedule tables and the RNG draw order stay on the host exactly
+as in the reference; each UNet evaluation with its update (two UNet branches + CFG combine + x_{t-1} update) is one
+native call.
 """
 from __future__ import annotations
 
@@ -8,6 +9,8 @@ from typing import Callable, List, Optional
 
 import numpy as np
 import torch
+
+from . import _lib
 
 
 def ddpm_tables(linear_start: float = 0.0015, linear_end: float = 0.0195, timesteps: int = 1000) -> dict:
@@ -88,5 +91,72 @@ class DDIMSampler:
                 m.masked_blend(img, x0, mask, qn, st)
             noise = noise_fn(i, "step") if noise_fn else torch.randn(shape, device=dev)   # ddim.py:351
             m.p_sample_ddim(img, st, noise, unconditional_guidance_scale, out=nxt)
+            img, nxt = nxt, img
+        return img
+
+
+class PLMSSampler(DDIMSampler):
+    """The reference ``PLMSSampler`` surface (plms.py:14-154) on the DDIM tables: ``make_schedule`` is DDIM's with eta
+    forced to 0 (plms.py:30), so every sigma is 0.  The loop keeps the reference's order of UNet evaluations, e_t
+    history and RNG draws; each evaluation is one native call (``model.p_sample_plms``).
+
+    With an unconditional dict and guidance != 1 the two branches are combined as DDIM does (e_u + s (e_c - e_u),
+    ddim.py:293-300).  The reference's own PLMS raises there on AudioLDM2's dict conditioning (torch.cat of dicts,
+    plms.py:290); this is the value it means to compute.  At guidance 1.0 the path is the reference's."""
+
+    def make_schedule(self, ddim_num_steps: int, ddim_discretize: str = "uniform", ddim_eta: float = 0.0, verbose: bool = False):
+        super().make_schedule(ddim_num_steps, ddim_discretize, 0.0, verbose)
+
+    @torch.no_grad()
+    def sample(self, S: int, batch_size: int, shape, conditioning=None, eta: float = 0.0, mask=None, x0=None,
+               unconditional_guidance_scale: float = 1.0, unconditional_conditioning=None, x_T=None,
+               noise_fn: Optional[Callable[[int, str], torch.Tensor]] = None, verbose: bool = False,
+               quantize_x0: bool = False, temperature: float = 1.0, noise_dropout: float = 0.0, score_corrector=None,
+               **kwargs):
+        """plms.py:92-154.  ``eta`` is accepted and ignored, as the reference ignores it.  ``noise_fn(i, kind)`` as in
+        DDIMSampler.sample: "q" once per masked step, then one "step" draw per update (two at the first step).  The
+        options AudioLDM2 never sets raise unless left at their defaults."""
+        if quantize_x0 or temperature != 1.0 or noise_dropout != 0.0 or score_corrector is not None or \
+                kwargs.get("ddim_use_original_steps") or kwargs.get("timesteps") is not None:
+            raise NotImplementedError("PLMS: quantize_x0, temperature, noise_dropout, score_corrector, timesteps and "
+                                      "ddim_use_original_steps are not part of the AudioLDM2 sampling path")
+        self.make_schedule(ddim_num_steps=S, ddim_eta=eta, verbose=verbose)
+        C_, T, F_ = shape
+        samples = self.plms_sampling(conditioning, (batch_size, C_, T, F_), x_T=x_T, mask=mask, x0=x0,
+                                     unconditional_guidance_scale=unconditional_guidance_scale,
+                                     unconditional_conditioning=unconditional_conditioning, noise_fn=noise_fn)
+        return samples, None
+
+    @torch.no_grad()
+    def plms_sampling(self, cond, shape, x_T=None, mask=None, x0=None, unconditional_guidance_scale: float = 1.0,
+                      unconditional_conditioning=None, noise_fn=None):
+        """plms.py:157-258 -- the hot loop.  e_t values live in four device buffers that rotate by reference: the
+        three the reference holds in old_eps (most recent first) and the one being written."""
+        m = self.model
+        dev = m.device
+        img = torch.randn(shape, device=dev) if x_T is None else x_T.to(dev).contiguous().clone()   # plms.py:180
+        single = unconditional_conditioning is None or unconditional_guidance_scale == 1.0     # plms.py:282-286
+        m.set_conditioning(cond, None if single else unconditional_conditioning)
+        g = unconditional_guidance_scale
+        step_noise = lambda i: noise_fn(i, "step") if noise_fn else torch.randn(shape, device=dev)   # plms.py:334
+        ring = [torch.empty(shape, dtype=torch.float32, device=dev) for _ in range(4)]
+        held: List[torch.Tensor] = []                   # old_eps, most recent first
+        nxt = torch.empty_like(img)
+        n = len(self.steps)
+        for i, st in enumerate(self.steps):
+            t_next = self.steps[min(i + 1, n - 1)]["t"]                                    # plms.py:215-220
+            if mask is not None:                                                           # plms.py:222-227
+                qn = noise_fn(i, "q") if noise_fn else torch.randn_like(x0)
+                m.masked_blend(img, x0, mask, qn, st)
+            e_t = next(r for r in ring if all(r is not h for h in held))
+            if not held:                                # plms.py:341-345: improved Euler through x' at t_next
+                step_noise(i)
+                m.p_sample_plms(img, st["t"], img, [], 1, st, g, e_t_out=e_t, out=nxt)
+                step_noise(i)
+                m.p_sample_plms(nxt, t_next, img, [e_t], _lib.PLMS_AVERAGE, st, g, out=nxt)
+            else:
+                step_noise(i)
+                m.p_sample_plms(img, st["t"], img, held, len(held) + 1, st, g, e_t_out=e_t, out=nxt)
+            held = [e_t] + held[:2]                                                        # plms.py:246-248
             img, nxt = nxt, img
         return img

@@ -16,6 +16,8 @@
  *       latent_diffusion/models/ddim.py:298-300,339-354
  *   masked blend + q_sample                                      aldm_ddim_step (mask != NULL)
  *       models/ddim.py:226-231, models/ddpm.py:430-436
+ *   PLMSSampler.p_sample_plms CFG combine + e' + x_{t-1} update  aldm_plms_step (one call per UNet evaluation;
+ *       latent_diffusion/models/plms.py:288-292,319-360            the first step takes two)
  *   LatentDiffusion.decode_first_stage -> AutoencoderKL.decode   aldm_program_run(vae-decoder program)
  *       models/ddpm.py:922-926, latent_encoder/autoencoder.py:111-117,
  *       modules/diffusionmodules/model.py:653-686
@@ -59,7 +61,7 @@
 extern "C" {
 #endif
 
-#define ALDM_ABI_VERSION 12
+#define ALDM_ABI_VERSION 13
 #define ALDM_MAX_TAPS 16
 
 enum {
@@ -219,6 +221,21 @@ int aldm_timestep_embedding(const int64_t* t, int32_t B, int32_t dim, const floa
 int aldm_ddim_step(const float* x, const float* eps_uncond, const float* eps_cond, const float* noise,
                    float* x_prev, float* pred_x0, int64_t n_total,
                    float a_t, float a_prev, float sigma_t, float sqrt_one_minus_at, float guidance,
+                   void* stream);
+
+/* PLMS step (plms.py:341-358), sigma = 0 (make_schedule forces eta = 0, plms.py:30): e_t = e_u + guidance*(e_c - e_u);
+ * e' from `order`:
+ *   1                  e' = e_t                                   (first evaluation of the first step)
+ *   2, 3, 4            Adams-Bashforth over e_t and order-1 held values, held1 the most recent:
+ *                      (3 e_t - h1) / 2, (23 e_t - 16 h1 + 5 h2) / 12, (55 e_t - 59 h1 + 37 h2 - 9 h3) / 24
+ *   ALDM_PLMS_AVERAGE  e' = (held1 + e_t) / 2, held1 = the first evaluation's e_t (second evaluation of the first step)
+ * then pred_x0 = (x - sqrt_one_minus_at*e') / sqrt(a_t), x_prev = sqrt(a_prev)*pred_x0 + sqrt(1-a_prev)*e', every
+ * operation rounded in the reference's order.  e_t_out (NULL: not stored; must be NULL with ALDM_PLMS_AVERAGE) receives
+ * e_t, the value the reference keeps in old_eps.  Unused held pointers may be NULL; pred_x0 may be NULL. */
+enum { ALDM_PLMS_AVERAGE = 0 };
+int aldm_plms_step(const float* x, const float* eps_uncond, const float* eps_cond, const float* held1,
+                   const float* held2, const float* held3, int32_t order, float* e_t_out, float* x_prev,
+                   float* pred_x0, int64_t n_total, float a_t, float a_prev, float sqrt_one_minus_at, float guidance,
                    void* stream);
 
 /* img = (sqrt_acp*x0 + sqrt_1m_acp*q_noise)*mask + (1-mask)*img; mask is [B,1,T,F] broadcast over C */
@@ -530,6 +547,8 @@ void aldm_program_destroy(aldm_program* p);
  *   aldm_engine_set_conditioning  <- DiffusionWrapper.forward's cond-dict unpacking (ddpm.py:1821-1879), once per call
  *   aldm_engine_unet_eps          <- the two self.model.apply_model(x, t, c) calls of p_sample_ddim (ddim.py:293-296)
  *   aldm_engine_ddim_step         <- DDIMSampler.p_sample_ddim as a whole (ddim.py:265-355): UNet x2 + CFG + update
+ *   aldm_engine_plms_step         <- one get_model_output + get_x_prev_and_pred_x0 of PLMSSampler.p_sample_plms
+ *                                    (plms.py:281-358): UNet x2 + CFG + e' + update; the first step is two calls
  *   aldm_engine_vae_decode        <- LatentDiffusion.decode_first_stage (ddpm.py:922-926)
  *   aldm_engine_vocoder           <- first_stage_model.vocoder(mel) in mel_spectrogram_to_waveform (ddpm.py:928-939)
  *   aldm_engine_vae_encode        <- encode_first_stage (ddpm.py:941-943), moments out
@@ -591,6 +610,13 @@ int aldm_engine_unet_eps(aldm_engine* e, const float* x, int64_t t, float* eps_u
 /* x_prev (and pred_x0 unless NULL) [B, C, T, F]; scalars as in aldm_ddim_step */
 int aldm_engine_ddim_step(aldm_engine* e, const float* x, int64_t t, const float* noise, float a_t, float a_prev,
                           float sigma_t, float sqrt_one_minus_at, float guidance, float* x_prev, float* pred_x0,
+                          void* stream);
+/* UNet pair on x_in at t, then aldm_plms_step per lane with x = x_base (x_in itself except for the first step's
+ * second evaluation, whose update starts again from that step's input).  held*, e_t_out, x_prev, pred_x0: [B, C, T, F]
+ * caller buffers (the e_t history ring is the caller's); x_prev may alias x_in but not x_base. */
+int aldm_engine_plms_step(aldm_engine* e, const float* x_in, int64_t t, const float* x_base, const float* held1,
+                          const float* held2, const float* held3, int32_t order, float* e_t_out, float a_t,
+                          float a_prev, float sqrt_one_minus_at, float guidance, float* x_prev, float* pred_x0,
                           void* stream);
 int aldm_engine_vae_decode(aldm_engine* e, const float* z, float* mel, void* stream);
 int aldm_engine_vocoder(aldm_engine* e, const float* mel, float* wave, void* stream);
