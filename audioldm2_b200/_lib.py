@@ -17,7 +17,8 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libaldm_b200.so")
 SOURCES = ["gemm.cu", "prep.cu", "attention.cu", "elementwise.cu", "stft.cu", "program.cu", "engine_abi.cu", "microbench.cu",
-           "cond/seqgen.cu", "text/t5.cu", "clap/clap_text.cu", "audio/htsat.cu", "sampler/plms.cu"]
+           "cond/seqgen.cu", "text/t5.cu", "clap/clap_text.cu", "audio/htsat.cu", "sampler/plms.cu",
+           "sampler/style.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
@@ -25,7 +26,7 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-
 NVCC = shutil.which("nvcc") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
 
 MAX_TAPS = 16
-ABI_VERSION = 13
+ABI_VERSION = 14
 
 # enums (keep in sync with the header; checked by tests/test_abi.py against the header text)
 GEMM_TC, GEMM_SIMT, GEMM_TC_V1 = 0, 1, 2
@@ -312,6 +313,7 @@ def lib() -> C.CDLL:
         "aldm_timestep_embedding": (i32, [vp, i32, i32, vp, vp, vp, vp]),
         "aldm_ddim_step": (i32, [vp, vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, vp]),
         "aldm_plms_step": (i32, [vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, i64, f32, f32, f32, f32, vp]),
+        "aldm_stochastic_encode": (i32, [vp, vp, vp, i64, f32, f32, vp, vp]),
         "aldm_masked_blend": (i32, [vp, vp, vp, vp, i32, i32, i32, f32, f32, vp]),
         "aldm_transpose_chw": (i32, [vp, vp, i32, i32, i32, i32, vp]),
         "aldm_posterior_sample": (i32, [vp, vp, vp, i32, i32, i32, f32, vp]),
@@ -363,7 +365,7 @@ EXPORTED = ["aldm_gemm", "aldm_gemm_variant", "aldm_gemm_a_mode", "aldm_prep", "
             "aldm_t5_embed", "aldm_t5_rmsnorm", "aldm_t5_attention", "aldm_t5_gate",
             "aldm_clap_embed", "aldm_clap_layernorm", "aldm_clap_attention", "aldm_clap_gelu", "aldm_clap_head",
             "aldm_htsat_logmel", "aldm_htsat_patch", "aldm_htsat_window_attention", "aldm_htsat_merge", "aldm_htsat_head",
-            "aldm_timestep_embedding", "aldm_ddim_step", "aldm_plms_step", "aldm_masked_blend", "aldm_transpose_chw",
+            "aldm_timestep_embedding", "aldm_ddim_step", "aldm_plms_step", "aldm_stochastic_encode", "aldm_masked_blend", "aldm_transpose_chw",
             "aldm_posterior_sample", "aldm_stft_mel", "aldm_program_create", "aldm_program_run",
             "aldm_program_run_range", "aldm_program_capture", "aldm_program_replay",
             "aldm_program_num_launches", "aldm_program_is_captured", "aldm_program_destroy", "aldm_engine_create",

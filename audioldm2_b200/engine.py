@@ -105,6 +105,21 @@ def ddim_step(x, eps_u, eps_c, noise, x_prev, a_t, a_prev, sigma_t, sqrt_one_min
     return x_prev
 
 
+def stochastic_encode(x0, noise, c0: float, c1: float, clip_flag=None, out=None):
+    """aldm_stochastic_encode: c0 * x0' + c1 * noise (ddim.py:434-449), x0' = clip(x0, -10, 10) when the device int32
+    ``clip_flag`` is non-zero (AudioLDM 1's latent guard; None: no guard)."""
+    L = _lib.lib()
+    out = torch.empty_like(x0) if out is None else out
+    for t in (x0, noise, out):
+        assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.shape == x0.shape
+    if clip_flag is not None:
+        assert clip_flag.is_cuda and clip_flag.dtype == torch.int32 and clip_flag.numel() == 1
+    _lib.check(L.aldm_stochastic_encode(x0.data_ptr(), noise.data_ptr(), out.data_ptr(), x0.numel(), c0, c1,
+                                        clip_flag.data_ptr() if clip_flag is not None else None, _stream_ptr()),
+               "stochastic_encode")
+    return out
+
+
 def masked_blend(img, x0, mask, q_noise, sqrt_acp, sqrt_1m_acp):
     L = _lib.lib()
     B, Cc, T, Fq = img.shape

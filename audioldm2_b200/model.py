@@ -8,6 +8,7 @@ pipeline read like the reference:
     mel_spectrogram_to_waveform(mel)         ddpm.py:928-939
     encode_first_stage(x) (+ posterior)      ddpm.py:941-943, 793-802
     q_sample / masked blend                  ddpm.py:430-436, ddim.py:226-231
+    stochastic_encode (style transfer)       ddim.py:434-449
 
 plus ``p_sample_ddim`` (ddim.py:265-355) fused into one native step, and each UNet evaluation of ``p_sample_plms``
 (plms.py:260-360) with its update as one native step.  Conditioning is either the
@@ -29,7 +30,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import _lib, arch, engine, plan
+from . import _lib, arch, engine, parallel, plan
 from .sampler import DDIMSampler, PLMSSampler, ddpm_tables
 
 
@@ -378,6 +379,11 @@ class NativeLatentDiffusion:
             "engine_plms_step")
         return out
 
+    def stochastic_encode(self, x0, noise, c0: float, c1: float, clip_flag=None):
+        """The arithmetic of DDIMSampler.stochastic_encode (ddim.py:434-449) with AudioLDM 1's guard word -- one native
+        pass, no host synchronisation."""
+        return engine.stochastic_encode(x0, noise, c0, c1, clip_flag)
+
     def masked_blend(self, img, x0, mask, q_noise, st: dict):
         return engine.masked_blend(img, x0, mask, q_noise, st["sqrt_acp_t"], st["sqrt_1m_acp_t"])
 
@@ -433,6 +439,29 @@ class NativeLatentDiffusion:
         z = self.generate_latent(cond, uncond, ddim_steps, guidance, eta, x_T, noise_fn, mask, x0, use_plms)
         mel = self.decode_first_stage(z)
         return self.mel_spectrogram_to_waveform(mel)
+
+    @torch.no_grad()
+    def style_transfer_latent(self, x0, cond: dict, uncond: Optional[dict], t_enc: int, ddim_steps: int = 200,
+                              guidance: float = 2.5, clip_flag=None, noise=None, noise_fn=None):
+        """AudioLDM 1's style_transfer from the initial latent ``x0`` on: make_schedule(ddim_steps, eta=1.0),
+        stochastic_encode at index ``t_enc`` (one draw, or ``noise``), then decode with indices t_enc - 1, ..., 0 (one
+        draw per step, or ``noise_fn(i, "step")``).  ``clip_flag``: the device guard word of
+        parallel.latent_guard_flag; None makes it from ``x0`` (the whole batch of a single-process call)."""
+        sampler = DDIMSampler(self)
+        sampler.make_schedule(ddim_num_steps=ddim_steps, ddim_eta=1.0)
+        x0 = x0.to(self.device, torch.float32).contiguous()
+        if clip_flag is None:
+            clip_flag = parallel.guard_decision(parallel.guard_flags(x0))
+        z_enc = sampler.stochastic_encode(x0, t_enc, noise=noise, clip_flag=clip_flag)
+        return sampler.decode(z_enc, cond, t_enc, unconditional_guidance_scale=guidance, unconditional_conditioning=uncond,
+                              noise_fn=noise_fn)
+
+    @torch.no_grad()
+    def style_transfer_waveform(self, x0, cond: dict, uncond: Optional[dict], t_enc: int, ddim_steps: int = 200,
+                                guidance: float = 2.5, clip_flag=None, noise=None, noise_fn=None):
+        """style_transfer_latent, then the whole latent decoded and vocoded as generate_batch does."""
+        z = self.style_transfer_latent(x0, cond, uncond, t_enc, ddim_steps, guidance, clip_flag, noise, noise_fn)
+        return self.mel_spectrogram_to_waveform(self.decode_first_stage(z))
 
     def launches_per_step(self) -> int:
         return self.lanes * (self.unet.num_launches("step") + 1 + 1)      # + timestep fill + K6, per lane

@@ -118,6 +118,31 @@ def max_over_ranks(value: float, device) -> float:
     return float(t.item())
 
 
+def guard_flags(x: torch.Tensor) -> torch.Tensor:
+    """The two inputs of AudioLDM 1's latent guard (``torch.max(torch.abs(x)) > 1e2`` then clip to [-10, 10]), made on
+    x's device without a host synchronisation: int32 [over, has_nan], over = max |x| > 100 (strict) and has_nan = any
+    NaN in x.  A NaN makes the reference's max NaN, so it must veto the clip."""
+    return torch.stack([torch.amax(torch.abs(x)) > 1e2, torch.isnan(x).any()]).to(torch.int32)
+
+
+def reduce_guard_flags(flags: torch.Tensor) -> torch.Tensor:
+    """guard_flags of every rank's rows combined with MAX, in place: one two-word collective per call, after which every
+    rank holds the flags of the whole batch and makes the single-process decision.  No-op in a single process."""
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        dist.all_reduce(flags, op=dist.ReduceOp.MAX)
+    return flags
+
+
+def guard_decision(flags: torch.Tensor) -> torch.Tensor:
+    """int32 [1] on the flags' device: 1 = clip (over and no NaN), the guard word aldm_stochastic_encode reads."""
+    return (flags[0] * (1 - flags[1])).reshape(1).to(torch.int32).contiguous()
+
+
+def latent_guard_flag(x: torch.Tensor) -> torch.Tensor:
+    """AudioLDM 1's guard decision for the whole batch of the call (all ranks' rows in a sharded run)."""
+    return guard_decision(reduce_guard_flags(guard_flags(x)))
+
+
 def barrier():
     if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
         dist.barrier()

@@ -36,6 +36,7 @@ import numpy as np
 import torch
 
 from . import arch, engine, frontend, model, parallel, synth
+from . import sampler as sampler_mod
 from .utils import seed_everything
 
 
@@ -435,22 +436,26 @@ class NativeAudioLDM2:
         """Every rank runs the same call with the same seed; prompts are cut into contiguous shards, the noise of the
         single-process latent batch (rows i + k * B) is drawn in full on every rank and sliced, and the selected waveforms are
         all-gathered at the end.  Results equal the single-process call row for row."""
+        local, glob, cond_l = self._shard_view(shard, batch, n_gen)
+        out = self._generate_local(local, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, glob, cond_l, use_plms)
+        full = parallel.all_gather_rows(torch.from_numpy(out).to(self.device), len(batch["text"]))
+        return self._egress(full)
+
+    def _shard_view(self, shard, batch, n_gen):
+        """This rank's part of a sharded call: (its prompts' batch, (B, its latent rows of the whole call), its rows of the
+        whole call's conditioning).  The candidates of prompt i sit at rows i + k * B."""
         _, _, lo, hi = shard
         B = len(batch["text"])
         local = {k: (v[lo:hi] if (torch.is_tensor(v) or isinstance(v, list)) and len(v) == B else v) for k, v in batch.items()}
         rows = [i + k * B for k in range(n_gen) for i in range(lo, hi)]
-        # conditioning of the whole call, this rank's rows: made by _generate_local after the posterior draw, as in one process
+        # conditioning of the whole call, this rank's rows: made after the posterior draw, as in one process
         cond_l = lambda: self._sharded_conditioning(batch, lo, hi)
-        out = self._generate_local(local, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, (B, rows), cond_l, use_plms)
-        full = parallel.all_gather_rows(torch.from_numpy(out).to(self.device), B)
-        return self._egress(full)
+        return local, (B, rows), cond_l
 
-    def _generate_local(self, batch, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, glob, cond_rows=None,
-                        use_plms=False):
-        masked = tmask is not None
+    def _encode_front(self, batch, n_gen, glob, eng, encode: bool):
+        """The front half shared by generation and the audio-to-audio calls, up to the conditioning: the posterior draw,
+        the CUDA noise of a sharded call, and the encoder pass when ``encode`` -> (x0 or None, x_T, noise_fn)."""
         B = len(batch["text"])
-        Bl = B * n_gen
-        eng = self.engine(Bl, with_encoder=masked)
         C_, T, F_ = eng.latent
         # get_input -> encode_first_stage -> posterior.sample() (ddpm.py:845-846): a CPU torch.randn of the latent shape
         # (distributions.py:38).  Plain text_to_audio encodes an all-zero fbank only to read z.shape[0]; that encoder pass is
@@ -464,12 +469,24 @@ class NativeAudioLDM2:
             noise_fn = parallel.ShardedNoise(Bg * n_gen, 0, 0, (C_, T, F_), self.device, rows=rows,
                                              generator=torch.cuda.default_generators[self.device.index or 0])
             x_T = noise_fn.x_T()
-        mask = x0 = None
-        if masked:
+        x0 = None
+        if encode:
             fbank = torch.as_tensor(batch["log_mel_spec"], dtype=torch.float32)           # [B, T', F']
             mel = _tile(fbank[:, None], n_gen).to(self.device)                            # torch.cat([z] * n_gen) (ddpm.py:1651)
             mom = eng.encode_first_stage_moments(mel)
             x0 = eng.get_first_stage_encoding(mom, _tile(post_noise, n_gen))
+        return x0, x_T, noise_fn
+
+    def _generate_local(self, batch, ddim_steps, ddim_eta, n_gen, guidance, uncond, tmask, fmask, glob, cond_rows=None,
+                        use_plms=False):
+        masked = tmask is not None
+        B = len(batch["text"])
+        Bl = B * n_gen
+        eng = self.engine(Bl, with_encoder=masked)
+        C_, T, F_ = eng.latent
+        x0, x_T, noise_fn = self._encode_front(batch, n_gen, glob, eng, masked)
+        mask = None
+        if masked:
             mask = torch.ones(Bl, T, F_, device=self.device)                              # ddpm.py:1611-1617
             mask[:, int(T * tmask[0]):int(T * tmask[1]), :] = 0
             mask[:, :, int(F_ * fmask[0]):int(F_ * fmask[1])] = 0
@@ -496,6 +513,34 @@ class NativeAudioLDM2:
             similarity = self.ranker(torch.from_numpy(waveform).squeeze(1), texts)
             waveform, _ = select_best(waveform, similarity, B)
         return waveform
+
+    # ---- style transfer (AudioLDM 1's style_transfer on AudioLDM2's primitives) ---------------------------------------
+    @torch.no_grad()
+    def generate_batch_style_transfer(self, batch, transfer_strength, ddim_steps=200, unconditional_guidance_scale=1.0,
+                                      unconditional_conditioning=None):
+        """The recording in ``batch["log_mel_spec"]`` encoded to its latent (one CPU posterior draw), AudioLDM 1's latent
+        guard, the conditioning of ``batch["text"]``, then DDIMSampler.stochastic_encode at t_enc = int(transfer_strength
+        * ddim_steps) (one CUDA draw) and decode over indices t_enc - 1, ..., 0 (one CUDA draw per step), decoder and
+        vocoder -> np.ndarray [B, 1, samples].  In a sharded call each rank runs its prompts' rows with the whole call's
+        draws, the guard's two flags are all-reduced once, and the waveforms are all-gathered at the end."""
+        t_enc = sampler_mod.transfer_steps(transfer_strength, ddim_steps, self.cfg["timesteps"])
+        B = len(batch["text"])
+        shard = parallel.current_shard(B)
+        local, glob, cond_l = (batch, None, None) if shard is None else self._shard_view(shard, batch, 1)
+        wave = self._style_transfer_local(local, ddim_steps, t_enc, unconditional_guidance_scale,
+                                          unconditional_conditioning, glob, cond_l)
+        return self._egress(parallel.all_gather_rows(wave, B))
+
+    def _style_transfer_local(self, batch, ddim_steps, t_enc, guidance, uncond, glob, cond_rows=None):
+        B = len(batch["text"])
+        eng = self.engine(B, with_encoder=True)
+        x0, noise, noise_fn = self._encode_front(batch, 1, glob, eng, True)
+        clip_flag = parallel.latent_guard_flag(x0)           # decided on the device: no synchronisation before the UNet
+        cond = cond_rows() if cond_rows is not None else self.conditioning(batch)
+        if guidance != 1.0:
+            uncond = self.unconditioning(B, uncond)
+        return eng.style_transfer_waveform(x0, cond, uncond, t_enc, ddim_steps=ddim_steps, guidance=guidance,
+                                           clip_flag=clip_flag, noise=noise, noise_fn=noise_fn)
 
 
 def build_model(ckpt_path=None, config=None, device=None, model_name="audioldm2-full", *, synthetic: Optional[bool] = None,
@@ -636,3 +681,44 @@ def super_resolution_and_inpainting(latent_diffusion, text, transcription="", or
             duration=duration, time_mask_ratio_start_and_end=time_mask_ratio_start_and_end,
             freq_mask_ratio_start_and_end=freq_mask_ratio_start_and_end, use_plms=use_plms)
     return waveform_out
+
+
+def round_up_duration(duration):
+    """pipeline.py:124-125: the duration, in steps of 2.5 s, that a recording of ``duration`` seconds is generated at."""
+    return int(round(duration / 2.5) + 1) * 2.5
+
+
+def style_transfer_sizes(cfg: dict, duration: float):
+    """(latent frames, mel frames) of style transfer at ``duration`` s: int(duration * latent_t_per_second), times the
+    VAE's 2 ** (len(ch_mult) - 1) -- 1024 mel frames at 10 s for both 16 kHz and 48 kHz, AudioLDM 1's int(duration *
+    102.4) at 16 kHz.  ValueError unless the latent length is a multiple of 8 (the UNet's three stride-2 levels)."""
+    latent_t = int(duration * cfg["latent_t_per_second"])
+    if latent_t % 8 != 0:
+        raise ValueError(f"duration {duration} s gives {latent_t} latent frames; the UNet needs a multiple of 8 "
+                         f"(durations in steps of {8 / cfg['latent_t_per_second']:g} s)")
+    return latent_t, latent_t * 2 ** (len(cfg["vae"]["ch_mult"]) - 1)
+
+
+def style_transfer(latent_diffusion, text, original_audio_file_path, transfer_strength, seed=42, duration=10, batchsize=1,
+                   guidance_scale=2.5, ddim_steps=200, config=None, *, waveform=None, waveform_sr=None):
+    """Audio-to-audio style transfer, AudioLDM 1's ``style_transfer`` on this engine: the recording's mel is encoded to
+    its latent, noised to DDIM index t_enc = int(transfer_strength * ddim_steps) and denoised over t_enc steps under
+    ``text`` (a prompt, or a list of ``batchsize`` prompts) -> np.ndarray [batchsize, 1, samples] float32.  A duration
+    longer than the recording becomes round_up_duration(its length).  ``waveform`` (+ ``waveform_sr``, keyword only)
+    replaces the file read.  ``config`` is accepted and unused, as in super_resolution_and_inpainting.  ValueError
+    before any draw when t_enc is outside [0, schedule length) or the latent length is not a multiple of 8."""
+    cfg = latent_diffusion.cfg
+    if waveform is None:
+        waveform, waveform_sr = frontend.read_wav(original_audio_file_path)
+    audio_duration = len(np.reshape(waveform, -1)) / float(waveform_sr or cfg["sampling_rate"])
+    if duration > audio_duration:
+        duration = round_up_duration(audio_duration)
+    seed_everything(int(seed))
+    latent_t, mel_frames = style_transfer_sizes(cfg, duration)
+    sampler_mod.transfer_steps(transfer_strength, ddim_steps, cfg["timesteps"])
+    mel, _ = wav_to_fbank(latent_diffusion, target_length=mel_frames, waveform=waveform, sr=waveform_sr)
+    batch = make_batch_for_text_to_audio(text, fbank=mel[None, ...], batchsize=batchsize)
+    latent_diffusion.latent_t_size = latent_t
+    with torch.no_grad():
+        return latent_diffusion.generate_batch_style_transfer(batch, transfer_strength, ddim_steps=ddim_steps,
+                                                              unconditional_guidance_scale=guidance_scale)

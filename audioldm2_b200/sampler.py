@@ -1,7 +1,7 @@
 """Host-side DDIM and PLMS schedulers: mirror ``DDIMSampler`` (latent_diffusion/models/ddim.py) and ``PLMSSampler``
 (latent_diffusion/models/plms.py) -- the Python loop, the schedule tables and the RNG draw order stay on the host exactly
 as in the reference; each UNet evaluation with its update (two UNet branches + CFG combine + x_{t-1} update) is one
-native call.
+native call.  ``DDIMSampler.stochastic_encode`` / ``decode`` serve style transfer.
 """
 from __future__ import annotations
 
@@ -20,6 +20,35 @@ def ddpm_tables(linear_start: float = 0.0015, linear_end: float = 0.0195, timest
     f32 = lambda a: torch.tensor(a, dtype=torch.float32)
     return dict(betas=f32(betas), alphas_cumprod=f32(ac), alphas_cumprod_prev=f32(np.append(1.0, ac[:-1])),
                 sqrt_alphas_cumprod=f32(np.sqrt(ac)), sqrt_one_minus_alphas_cumprod=f32(np.sqrt(1.0 - ac)))
+
+
+def ddim_schedule_length(S: int, num_timesteps: int = 1000) -> int:
+    """len(make_ddim_timesteps("uniform", S, T)) (util.py:55-75): range(0, T, T // S), so S = 6 gives 7 entries."""
+    if int(S) < 1 or num_timesteps // int(S) < 1:
+        raise ValueError(f"ddim_steps={S} must be in [1, {num_timesteps}]")
+    return len(range(0, num_timesteps, num_timesteps // int(S)))
+
+
+def transfer_steps(transfer_strength: float, ddim_steps: int, num_timesteps: int = 1000) -> int:
+    """Style transfer's t_enc = int(transfer_strength * ddim_steps) (Python float arithmetic: int(0.29 * 100) == 28),
+    checked against the schedule: stochastic_encode gathers index t_enc of it, so 0 <= t_enc < its length, which for
+    S = 6 (7 entries) admits strength 1.0.  ValueError otherwise -- the reference fails later with an index error."""
+    n = ddim_schedule_length(ddim_steps, num_timesteps)
+    t_enc = int(transfer_strength * ddim_steps)
+    if not 0 <= t_enc < n:
+        raise ValueError(f"transfer_strength={transfer_strength} with ddim_steps={ddim_steps} gives t_enc={t_enc}; "
+                         f"it must lie in [0, {n - 1}], the indices of the {n}-entry DDIM schedule")
+    return t_enc
+
+
+def _single_index(t) -> int:
+    """The one timestep index of ``t`` (an int, or a tensor of equal entries as AudioLDM passes)."""
+    if torch.is_tensor(t):
+        v = t.reshape(-1)
+        if v.numel() == 0 or not bool((v == v[0]).all()):
+            raise NotImplementedError("stochastic_encode: one t for the whole batch (AudioLDM passes [t_enc] * B)")
+        return int(v[0])
+    return int(t)
 
 
 class DDIMSampler:
@@ -92,6 +121,54 @@ class DDIMSampler:
             noise = noise_fn(i, "step") if noise_fn else torch.randn(shape, device=dev)   # ddim.py:351
             m.p_sample_ddim(img, st, noise, unconditional_guidance_scale, out=nxt)
             img, nxt = nxt, img
+        return img
+
+    @torch.no_grad()
+    def stochastic_encode(self, x0, t, use_original_steps: bool = False, noise=None, *, clip_flag=None):
+        """ddim.py:434-449: sqrt(ddim_alphas)[t] * x0 + ddim_sqrt_one_minus_alphas[t] * noise, both coefficients fp32 as
+        the reference gathers them; ``noise`` is drawn with randn_like(x0) on the device when not given (one CUDA draw).
+        ``clip_flag`` (keyword only): a device int32 guard word; when non-zero x0 is clipped to [-10, 10] first (AudioLDM
+        1's latent guard, see parallel.latent_guard_flag).  One native pass."""
+        if use_original_steps:
+            raise NotImplementedError("stochastic_encode: use_original_steps is not part of AudioLDM's style transfer")
+        ti = _single_index(t)
+        n = len(self.ddim_timesteps)
+        if not 0 <= ti < n:
+            raise ValueError(f"stochastic_encode: t={ti} outside the {n}-entry DDIM schedule")
+        m = self.model
+        x0 = x0.to(m.device, torch.float32).contiguous()
+        noise = torch.randn_like(x0) if noise is None else noise.to(m.device, torch.float32).contiguous()
+        c0 = float(torch.sqrt(torch.as_tensor(self.ddim_alphas, dtype=torch.float32))[ti])
+        c1 = float(torch.as_tensor(self.ddim_sqrt_one_minus_alphas, dtype=torch.float32)[ti])
+        return m.stochastic_encode(x0, noise, c0, c1, clip_flag)
+
+    @torch.no_grad()
+    def decode(self, x_latent, cond, t_start: int, unconditional_guidance_scale: float = 1.0,
+               unconditional_conditioning=None, use_original_steps: bool = False, callback=None,
+               noise_fn: Optional[Callable[[int, str], torch.Tensor]] = None):
+        """ddim.py:451-491: p_sample_ddim at indices t_start - 1, ..., 0 -- the last t_start entries of ``steps`` -- with
+        one noise draw per step (``noise_fn(i, "step")`` or torch.randn on the device), as ddim_sampling's loop does.
+        t_start = 0 runs no step."""
+        if use_original_steps:
+            raise NotImplementedError("decode: use_original_steps is not part of AudioLDM's style transfer")
+        t_start = int(t_start)
+        if not 0 <= t_start <= len(self.steps):
+            raise ValueError(f"decode: t_start={t_start} outside [0, {len(self.steps)}]")
+        m = self.model
+        dev = m.device
+        img = x_latent.to(dev, torch.float32).contiguous().clone()
+        if t_start == 0:
+            return img
+        shape = tuple(img.shape)
+        single = unconditional_conditioning is None or unconditional_guidance_scale == 1.0     # ddim.py:284-285
+        m.set_conditioning(cond, None if single else unconditional_conditioning)
+        nxt = torch.empty_like(img)
+        for i, st in enumerate(self.steps[len(self.steps) - t_start:]):
+            noise = noise_fn(i, "step") if noise_fn else torch.randn(shape, device=dev)   # ddim.py:351
+            m.p_sample_ddim(img, st, noise, unconditional_guidance_scale, out=nxt)
+            img, nxt = nxt, img
+            if callback:
+                callback(i)
         return img
 
 

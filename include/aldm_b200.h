@@ -15,6 +15,8 @@
  *   DDIMSampler.p_sample_ddim CFG combine + x_{t-1} update       aldm_ddim_step
  *       latent_diffusion/models/ddim.py:298-300,339-354
  *   masked blend + q_sample                                      aldm_ddim_step (mask != NULL)
+ *   DDIMSampler.stochastic_encode (+ AudioLDM 1's latent guard)   aldm_stochastic_encode (style transfer)
+ *       latent_diffusion/models/ddim.py:434-449
  *       models/ddim.py:226-231, models/ddpm.py:430-436
  *   PLMSSampler.p_sample_plms CFG combine + e' + x_{t-1} update  aldm_plms_step (one call per UNet evaluation;
  *       latent_diffusion/models/plms.py:288-292,319-360            the first step takes two)
@@ -61,7 +63,7 @@
 extern "C" {
 #endif
 
-#define ALDM_ABI_VERSION 13
+#define ALDM_ABI_VERSION 14
 #define ALDM_MAX_TAPS 16
 
 enum {
@@ -237,6 +239,14 @@ int aldm_plms_step(const float* x, const float* eps_uncond, const float* eps_con
                    const float* held2, const float* held3, int32_t order, float* e_t_out, float* x_prev,
                    float* pred_x0, int64_t n_total, float a_t, float a_prev, float sqrt_one_minus_at, float guidance,
                    void* stream);
+
+/* DDIMSampler.stochastic_encode (ddim.py:434-449) of style transfer: out = c0*x0' + c1*noise, c0 = sqrt(ddim_alphas)[t],
+ * c1 = ddim_sqrt_one_minus_alphas[t] (fp32), the two products and the sum rounded one by one.  x0' = x0, or
+ * clip(x0, -10, 10) when clip_flag (a device int32; NULL: no guard) is non-zero: AudioLDM 1's latent guard, decided on
+ * the device so that no host synchronisation separates the VAE encoder from the first UNet step.  NaN passes through
+ * the clip.  out must not overlap x0, noise or clip_flag. */
+int aldm_stochastic_encode(const float* x0, const float* noise, float* out, int64_t n_total, float c0, float c1,
+                           const int32_t* clip_flag, void* stream);
 
 /* img = (sqrt_acp*x0 + sqrt_1m_acp*q_noise)*mask + (1-mask)*img; mask is [B,1,T,F] broadcast over C */
 int aldm_masked_blend(float* img, const float* x0, const float* mask, const float* q_noise,
